@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""bench.py -- tokens/sec of LLaMA-7B q4_0 greedy decode (n_batch = 1) on B200, BASELINE.json's metric.
+"""bench.py -- tokens/sec of LLaMA-7B q4_0 greedy decode (n_batch = 1) on H100, BASELINE.json's metric.
 
     python bench.py --gpus N --steps K --warmup W            # our arm
     python bench.py --impl reference --gpus N --steps K ...   # the reference's CPU path (rank 0 only)
     python bench.py --mode ingest                             # BASELINE configs[2]: prompt ingest, n_batch = 128 (tensor-core GEMM)
     python bench.py --size 13B --wtype q4_1                   # BASELINE configs[3]
+    python bench.py --dump-outputs DIR                        # also write the last timed step's outputs as DIR/<name>.npy
 
 A "step" is one decoded token = one pass of the hot path (7*32+1 quantised matvecs, 4 129 423 360 algorithmic weight bytes) over a
 synthetic random-weight 7B q4_0 model (N(0, 0.02^2), seed 0, GGJT file written once to $FASTLLAMA_BENCH_DIR or /tmp by a child
@@ -21,6 +22,8 @@ process).  Keys of the JSON line:
              thread sweep, best setting reported, bounded sample; runs in child processes that never load this repository's libraries
   parity     same prompt, greedy: the reference's token sequence and per-step logits against ours (7B q4_0, N = 1); under torchrun the
              ranks' logits are compared with each other and the tokens with the N = 1 run's (written next to the model file)
+  --dump-outputs DIR  after the timed steps: DIR/logits.npy, the float32 logits the caller of the timed path receives from its last
+             step (Model.get_logits_array()); the inputs (seeded synthetic model, fixed prompt, greedy) are the same on every run
   extra      further BASELINE configs measured in the same invocation (N = 1 only): 13B q4_1 decode, 7B prompt ingest n_batch = 128,
              7B decode at n_past ~ 256 and ~ 480, each with its own roofline object
 """
@@ -76,7 +79,7 @@ class _Stats(C.Structure):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -259,7 +262,7 @@ def cpu_reference(path: str, size: str, wtype_name: str, steps: int, n_parity: i
 # our arm
 # ---------------------------------------------------------------------------------------------------------------------
 class Backend:
-    """Handles to the three in-tree libraries; fails loudly without the CUDA library / a B200."""
+    """Handles to the three in-tree libraries; fails loudly without the CUDA library / an H100."""
 
     def __init__(self, local_rank: int):
         os.environ.setdefault("FASTLLAMA_DEVICE", str(local_rank))
@@ -343,26 +346,10 @@ def load_peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return p, "MEASURED_PEAKS.json (of measured)"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "B200_PROFILING.md fallback (of fallback)"
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet at 700 W, not measured (of fallback)"
 
 
-def committed_traffic():
-    """DRAM bytes per k_decode_token launch from the newest committed ncu --set full capture (NOT measured in this run)."""
-    best = None
-    pdir = os.path.join(ROOT, "profiles")
-    for name in sorted(os.listdir(pdir)) if os.path.isdir(pdir) else []:
-        if name.endswith("_ncu_token_kernel.json"):
-            best = name
-    if not best:
-        return None, None
-    try:
-        cap = json.load(open(os.path.join(pdir, best)))
-        return int(cap["dram_bytes_read"]) + int(cap["dram_bytes_write"]), f"from_committed_profile: profiles/{best} (ncu --set full, one launch; not re-measured in this run)"
-    except Exception:
-        return None, None
-
-
-def ingest_run(be: Backend, path: str, size: str, wtype_name: str, peaks, peak_src, batches: int = 2):
+def ingest_run(be: Backend, path: str, size: str, wtype_name: str, peaks, peak_src, batches: int = 2, dump_dir=None):
     """Prompt ingest with n_batch = 128: the prompt is batches*128 + 1 tokens, so ingest() evaluates `batches` full 128-token
     chunks (the last chunk, one token, is left to the first generate(); reference lib/bridge.cpp:213-232)."""
     m = be.model(path, n_batch=128)
@@ -378,6 +365,8 @@ def ingest_run(be: Backend, path: str, size: str, wtype_name: str, peaks, peak_s
     be.fl.check(be.fl.lib.fl_sync())
     t1 = time.perf_counter()
     s1 = be.stats()
+    if dump_dir:
+        dump_outputs(dump_dir, {"logits": m.get_logits_array()})
     evals = int(s1.n_evals - s0.n_evals)
     dev_s = (s1.total_device_us - s0.total_device_us) * 1e-6
     launches = int(be.fl.lib.fl_launch_count() - l0)
@@ -385,17 +374,17 @@ def ingest_run(be: Backend, path: str, size: str, wtype_name: str, peaks, peak_s
     flops = 2.0 * 128 * MATMUL_PARAMS[size]
     per_eval = dev_s / evals if evals else 0.0
     tf = flops / per_eval / 1e12 if per_eval else 0.0
-    peak_t = float(peaks.get("bf16_tflops_sustained", 1400.0))
+    peak_t = float(peaks.get("bf16_tflops_sustained", 989.0))
     algo = ALGO_BYTES_PER_TOKEN.get((size, wtype_name))
     res = {"metric": f"prompt tokens/sec LLaMA-{size} {wtype_name} ingest (n_batch=128)", "value": n_tok / dev_s if dev_s else 0.0, "unit": "tokens/s", "steps": evals,
            "ms_per_step": per_eval * 1e3, "config": {"workload": f"LLaMA-{size} {wtype_name} prompt ingest, n_batch=128, {evals} evals of 128 tokens at n_past 0..{n_tok - 128}, n_ctx=512"},
            "e2e": {"value": n_tok / (t1 - t0), "unit": "tokens/s", "h2d_bytes_per_step": 128 * 4, "d2h_bytes_per_step": 32000 * 4 + 4 * {"7B": 4096, "13B": 5120, "65B": 8192}[size]},
            "gpu_launches": launches,
            "roofline": {"bound": "tensor", "achieved": tf, "peak": peak_t, "unit": "TFLOP/s", "frac": tf / peak_t, "traffic": None,
-                        "kernel": "k_mul_mat_q_umma (tcgen05.mma kind::i8, one MMA per quant block into TMEM; exact fp32 block scaling on the CUDA cores) -- the whole eval "
+                        "kernel": "k_mul_mat_q_umma (wgmma.mma_async with 8-bit integer operands, one MMA per quant block into registers; exact fp32 block scaling on the CUDA cores) -- the whole eval "
                                   "(all 7*n_layer+1 GEMMs + attention + element-wise ops) is in the timed bracket",
                         "algorithmic_flops_per_step": flops, "peak_source": peak_src + " bf16_tflops_sustained (the MMAs are 8-bit integer; nominal i8 peak is 2x bf16)",
-                        "hbm_line": {"achieved_gbs": (algo / per_eval / 1e9) if (algo and per_eval) else None, "peak_gbs": float(peaks.get("hbm_gbs", 6650.0)),
+                        "hbm_line": {"achieved_gbs": (algo / per_eval / 1e9) if (algo and per_eval) else None, "peak_gbs": float(peaks.get("hbm_gbs", 3350.0)),
                                      "note": "weights read once per 128-token eval"}}}
     # continue into decode at n_past ~ 256: the KV cache now adds 2 * n_layer * n_past * n_embd * 4 bytes of reads per token
     extra_decode = []
@@ -415,7 +404,7 @@ def ingest_run(be: Backend, path: str, size: str, wtype_name: str, peaks, peak_s
             n_past_mid = (batches * 128 + 8) if target == 256 else 464 + 8
             kv = 2 * n_layer * n_past_mid * n_embd * 4
             # the first eval of the 16 is the pending prompt chunk; all are N = 1 here
-            rl = roofline_hbm(algo, cur["device_s"], cur["evals"], float(peaks.get("hbm_gbs", 6650.0)), peak_src + " hbm_gbs", TOKEN_KERNEL)
+            rl = roofline_hbm(algo, cur["device_s"], cur["evals"], float(peaks.get("hbm_gbs", 3350.0)), peak_src + " hbm_gbs", TOKEN_KERNEL)
             rl["kv_cache_bytes_per_token_not_in_achieved"] = kv
             rl["achieved_incl_kv_gbs"] = (algo + kv) / (cur["device_s"] / cur["evals"]) / 1e9
             extra_decode.append({"metric": f"tokens/sec LLaMA-{size} {wtype_name} decode (n_batch=1, greedy) at n_past ~{n_past_mid}", "value": cur["evals"] / cur["device_s"], "unit": "tokens/s",
@@ -443,8 +432,19 @@ def decode_run(be: Backend, path, size, wtype_name, steps, warmup, peaks, peak_s
     m.generate(lambda s: None, num_tokens=max(warmup - len(toks), 3), **GREEDY)       # >= 3 untimed warm-up steps on the graph-replay path
     r = timed_decode(be, m, steps, dist=dist, local_rank=local_rank)
     mode = int(be.ggml.ggml_b200_decode_mode())
+    last = {"logits": m.get_logits_array()}                      # what the caller receives from the last timed step
     m.close()
-    return r, mode, toks, (np.stack(logits) if logits else None)
+    return r, mode, toks, (np.stack(logits) if logits else None), last
+
+
+def dump_outputs(out_dir: str, arrays: dict):
+    """DIR/<name>.npy for every array, as float32 / float64 (the logits of one step: 128 KB)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        np.save(os.path.join(out_dir, f"{name}.npy"), a if a.dtype in (np.float32, np.float64) else a.astype(np.float64))
 
 
 def compare_parity(ref_tokens, ref_logits, our_tokens, our_logits):
@@ -480,7 +480,7 @@ def compare_parity(ref_tokens, ref_logits, our_tokens, our_logits):
             out["note"] = ("every activation is re-quantised to q8_0 before every matmul (reference lib/ggml.c:8105-8119): a dense relative perturbation d becomes "
                            "sqrt(d * step) after one quantised matmul (step = 1/127 of a block's amax), so one differing ulp anywhere settles at a few per cent of "
                            "max|logit| within a layer or two on this random-weight model; DESIGN.md section 5.  A prompt of 16 tokens or more goes through the "
-                           "tcgen05 GEMM, whose block terms are added in another fp32 order (FASTLLAMA_B200_INGEST=exact keeps the reference's order)")
+                           "wgmma GEMM, whose block terms are added in another fp32 order (FASTLLAMA_B200_INGEST=exact keeps the reference's order)")
     return out
 
 
@@ -497,6 +497,7 @@ def main():
     ap.add_argument("--parity-tokens", type=int, default=32)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the outputs of the last timed step as DIR/<name>.npy")
     ap.add_argument("--_gen", nargs=2, default=None, help=argparse.SUPPRESS)
     ap.add_argument("--_ref-worker", default=None, help=argparse.SUPPRESS)
     args = ap.parse_args()
@@ -518,7 +519,7 @@ def main():
     # identical in both arms (the driver compares it): what is measured, not how
     config = {"workload": workload, "prompt": PROMPT, "algorithmic_bytes_per_token": algo,
               "parallelism": "1 GPU" if args.gpus == 1 else f"tp{args.gpus} (one decode stream, tensor parallel)",
-              "l2": f"inputs ({(algo or 0) / 1e9:.2f} GB of weights per step) are {(algo or 0) / 126e6:.0f}x larger than L2; no flush needed"}
+              "l2": f"inputs ({(algo or 0) / 1e9:.2f} GB of weights per step) are {(algo or 0) / 50e6:.0f}x larger than L2; no flush needed"}
 
     # ---------------------------------------------------------------- reference arm (CPU, rank 0 only; no library of this repository in the timing process)
     if args.impl == "reference":
@@ -576,11 +577,13 @@ def main():
         dist.barrier()
     path = model_path(args.size, args.wtype)
     peaks, peak_src = load_peaks()
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))
 
     if args.mode == "ingest":
         assert world == 1, "--mode ingest is a single-GPU measurement"
-        res, extra_decode = ingest_run(be, path, args.size, args.wtype, peaks, peak_src, batches=max(1, min(3, args.steps)))
+        if args.steps > 3:
+            raise SystemExit("--mode ingest times at most 3 evals of 128 tokens (n_ctx = 512); pass --steps 1..3")
+        res, extra_decode = ingest_run(be, path, args.size, args.wtype, peaks, peak_src, batches=max(1, args.steps), dump_dir=args.dump_outputs)
         res.update({"n_gpus": 1, "warmup": 1, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic"})
         res["config"] = config
         res["device"] = be.props["name"]
@@ -604,9 +607,11 @@ def main():
                 ref_logits = np.load(lp)
         log(f"[bench] cpu_baseline: {cpu_baseline['value']:.2f} tokens/s on {cpu_baseline['cores']} threads")
 
-    r, decode_mode, our_tokens, our_logits = decode_run(be, path, args.size, args.wtype, args.steps, args.warmup, peaks, peak_src, dist=dist, local_rank=local_rank,
+    r, decode_mode, our_tokens, our_logits, last = decode_run(be, path, args.size, args.wtype, args.steps, args.warmup, peaks, peak_src, dist=dist, local_rank=local_rank,
                                                          parity_n=parity_n if (world == 1 or tp) else 0)
-    n_tok = r["tokens"]
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
+    n_tok = r["evals"]                                            # one eval per decoded token
     if n_tok < args.steps:
         log(f"[bench] rank {rank}: generation stopped after {n_tok} of {args.steps} tokens (EOS); rates use the tokens produced")
     wall, device_s = r["wall_s"], r["device_s"]
@@ -655,10 +660,9 @@ def main():
     from fastllama_b200.ggjt import LLAMA_SIZES
 
     n_embd_model = LLAMA_SIZES[args.size][0]
-    traffic, traffic_src = committed_traffic() if (headline and world == 1 and decode_mode == 2) else (None, None)
     if decode_mode == 2 and algo and r["evals"]:
         # per-GPU algorithmic bytes: the weights are sharded N ways under tensor parallelism (the LM head and all layers split evenly)
-        rl = roofline_hbm(algo / (world if tp else 1), device_s, r["evals"], peak, peak_src + " hbm_gbs", TOKEN_KERNEL, traffic, traffic_src)
+        rl = roofline_hbm(algo / (world if tp else 1), device_s, r["evals"], peak, peak_src + " hbm_gbs", TOKEN_KERNEL)
         if tp:
             rl["per_gpu"] = True
     else:
@@ -696,7 +700,7 @@ def main():
             extra.append({"metric": "prompt ingest n_batch=128", "error": repr(e)})
         try:
             p13 = ensure_model("13B", "q4_1")
-            r13, mode13, _, _ = decode_run(be, p13, "13B", "q4_1", 32, 5, peaks, peak_src)
+            r13, mode13, _, _, _ = decode_run(be, p13, "13B", "q4_1", 32, 5, peaks, peak_src)
             a13 = ALGO_BYTES_PER_TOKEN[("13B", "q4_1")]
             extra.append({"metric": "tokens/sec LLaMA-13B q4_1 decode (n_batch=1, greedy)", "value": r13["evals"] / r13["device_s"], "unit": "tokens/s", "steps": r13["evals"],
                           "ms_per_step": 1e3 * r13["device_s"] / r13["evals"], "e2e": {"value": r13["tokens"] / r13["wall_s"], "unit": "tokens/s"},

@@ -1,4 +1,4 @@
-"""In-tree build of the native libraries (nvcc cross-compiles sm_100a without a GPU)."""
+"""In-tree build of the native libraries (nvcc cross-compiles sm_90a without a GPU)."""
 from __future__ import annotations
 
 import os

@@ -1,4 +1,4 @@
-// fl_common.cuh -- block formats, PTX wrappers and error plumbing shared by the sm_100a kernels.
+// fl_common.cuh -- block formats, PTX wrappers and error plumbing shared by the sm_90a kernels.
 //
 // Block formats are the reference's on-disk / in-memory layouts and are kept byte for byte
 // (reference lib/ggml.c:590-626): q4_0 {f32 d; u8 qs[16]} 20 B, q4_1 {f32 d; f32 m; u8 qs[16]}
@@ -62,7 +62,7 @@ __device__ __forceinline__ int fl_dp4a_ss(uint32_t a_s8x4, uint32_t b_s8x4, int 
     return r;
 }
 
-// mbarrier (shared::cta) -- the async-copy completion mechanism of sm_90+/sm_100
+// mbarrier (shared::cta) -- the async-copy completion mechanism of sm_90
 __device__ __forceinline__ void fl_mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }

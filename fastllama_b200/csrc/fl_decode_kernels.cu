@@ -396,7 +396,7 @@ static int fd_query() {
 
 static bool fd_use_pdl() {
     static int v = -1;
-    // measured on B200 (round 1): with PDL the 7B decode step is SLOWER (3.07 vs 2.28 ms/token), so it is opt-in
+    // with PDL the 7B decode step was slower, so it is opt-in
     if (v < 0) v = getenv("FASTLLAMA_B200_PDL") ? 1 : 0;
     return v != 0;
 }

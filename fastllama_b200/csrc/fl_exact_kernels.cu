@@ -3,7 +3,7 @@
 //   k_yx_prepare        q8_0 blocks -> prepared 80-byte blocks (per-quad words and biases)
 //   k_mul_mat_q_ref     q4_0 / q4_1 weights x prepared activations, any M, K, N: 8 rows per warp, 4 lanes per row, blocks in
 //                       order, NC activation columns per pass.  This is the general path (small prompts, shapes the token
-//                       kernel or the tcgen05 GEMM do not take, FASTLLAMA_B200_INGEST=exact); the decode step runs the same
+//                       kernel or the wgmma GEMM do not take, FASTLLAMA_B200_INGEST=exact); the decode step runs the same
 //                       arithmetic inside k_decode_token.
 //   k_mul_mat_f32_ref4  f32 x f32 mul_mat on strided 4-D views (attention scores K.Q and the value mix V.P of a multi-token
 //                       eval) in ggml_vec_dot_f32's order: lane l of a warp is element l of the reference's 32-float step.

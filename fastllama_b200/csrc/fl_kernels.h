@@ -44,8 +44,8 @@ int flk_rope(cudaStream_t st, const fl_view &t, int n_past, int n_dims, int mode
 int flk_cpy_f32(cudaStream_t st, const fl_view &src, const fl_view &dst);
 int flk_mul_mat_f32(cudaStream_t st, const fl_view &src0, const fl_view &src1, const fl_view &dst);
 
-// fl_umma_kernel.cu: N > 1 on the Blackwell tensor cores: one tcgen05.mma kind::i8 (M = 128, K = 32) per quant block into TMEM,
-// weights by TMA, exact fp32 block scaling by the epilogue warps.  nt_hint: column-tile width (0 = choose; 32 / 64 / 128)
+// fl_umma_kernel.cu: N > 1 on the Hopper tensor cores: one wgmma (M = 64, K = 32, 8-bit operands) per quant block into registers,
+// weights by TMA, exact fp32 block scaling by the same warpgroup.  nt_hint: column-tile width (0 = choose; 32 / 64; 128 is taken as 64)
 int flk_mul_mat_q_umma_supported(int type, const void *W, size_t w_row_stride, int M, int K, int N);
 int flk_mul_mat_q_umma(cudaStream_t st, int type, const void *W, size_t w_row_stride, int M, int K, const void *Yq8, int N, float *dst,
                        size_t dst_row_stride, int nt_hint);

@@ -16,8 +16,6 @@
 // block -- the same prepared layout the decode kernels use.  The -8 of q4_0 is folded in as
 // c[n][kb] = -8 * sum(q8), added to the integer result.
 //
-// tcgen05 is not used: the exact per-block scaling needs the s32 partial sum of every k-block, which
-// would mean draining TMEM after every K = 32 step (DESIGN.md section 8).
 #include "fl_common.cuh"
 #include "fl_kernels.h"
 

@@ -1,4 +1,4 @@
-// fl_quant_kernels.cu -- sm_100a kernels for the q4_0/q4_1 x q8_0 hot path.
+// fl_quant_kernels.cu -- sm_90a kernels for the q4_0/q4_1 x q8_0 hot path.
 //
 //   k_quantize_q8_0      activations -> q8_0 blocks      (reference lib/ggml.c:1299-1441, AVX2 semantics)
 //   k_quantize_q4_{0,1}  weights -> q4 blocks            (reference lib/ggml.c:630-664, :917-956)
@@ -567,10 +567,10 @@ int flk_mul_mat_q(cudaStream_t st, int type, const void *W, size_t wrs, int M, i
     FL_REQUIRE(((uintptr_t)W & 3) == 0 && (wrs & 3) == 0, "mul_mat_q: weight rows must be 4-byte aligned");
     if (M <= 0 || N <= 0) return 0;
     // impl 0 (what the graph executor passes): results carry the reference's bits -- the reference-order kernel of fl_exact_kernels.cu --
-    // except for multi-token evals of N >= 16 columns, which go to the tcgen05 GEMM (same per-block arithmetic, block terms added in
+    // except for multi-token evals of N >= 16 columns, which go to the wgmma GEMM (same per-block arithmetic, block terms added in
     // another fp32 order: within the stated budget, not bit-identical) unless FASTLLAMA_B200_INGEST=exact.
     // The other kernels stay selectable for measurements and their own tests: 1 plain, 2 TMA ring matvec, 3 mma.sync,
-    // 4-7 tcgen05 (column tile chosen / 32 / 64 / 128), 8 reference order.
+    // 4-7 wgmma (column tile chosen / 32 / 64 / 64), 8 reference order.
     if (impl == 0) {
         static const int umma_auto = getenv("FASTLLAMA_B200_UMMA") ? atoi(getenv("FASTLLAMA_B200_UMMA")) : 1;     // FASTLLAMA_B200_UMMA=0: no tensor-core path
         const char *ing = getenv("FASTLLAMA_B200_INGEST");               // read per call: tests and callers may switch it between evals

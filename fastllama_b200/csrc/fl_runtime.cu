@@ -1,5 +1,5 @@
 // fl_runtime.cu -- library state, memory, lookup tables and the extern "C" entry points of
-// include/fl_cuda.h.  No CPU compute path exists here: every entry point either runs the sm_100a
+// include/fl_cuda.h.  No CPU compute path exists here: every entry point either runs the sm_90a
 // kernels or fails loudly.
 #include <cuda_fp16.h>
 #include <dlfcn.h>
@@ -138,7 +138,7 @@ extern "C" int fl_init(int device) {
     FL_CUDA_OK(cudaSetDevice(device));
     cudaDeviceProp prop;
     FL_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-    FL_REQUIRE(prop.major == 10, "fl_init: built for sm_100a only, device %d is sm_%d%d (%s)", device, prop.major,
+    FL_REQUIRE(prop.major == 9 && prop.minor == 0, "fl_init: built for sm_90a only, device %d is sm_%d%d (%s)", device, prop.major,
                prop.minor, prop.name);
     FL_CUDA_OK(cudaStreamCreateWithFlags(&g.stream, cudaStreamNonBlocking));
     g.device = device;

@@ -2,7 +2,7 @@
 //
 // Why: with one kernel per matrix group the decode step is 160 launches of 3-18 us whose fixed costs
 // (launch, barrier init, prologue, first-tile latency, drain) leave HBM idle ~70 % of the time
-// (DESIGN.md section 4).  Here 148 CTAs (one per SM, co-resident by cooperative launch) walk a
+// (DESIGN.md section 4).  Here one CTA per SM (co-resident by cooperative launch) walk a
 // "program" of phases -- per layer: wq|wk|wv, attention, wo, w1|w3, w2; then the LM head -- separated
 // by grid-wide barriers, and each CTA's producer lane streams the weight tiles of ALL phases through one
 // mbarrier ring, running ahead of the consumers across phase boundaries: while the grid synchronises
@@ -147,7 +147,7 @@ __device__ __forceinline__ void tk_tag_wait(volatile uint32_t *tag, uint32_t wan
 // with ld.global.cg only.  Only the step in front of the attention needs it (q and the KV rows of all CTAs); every other
 // hand-over is a dataflow (LL) vector.
 __device__ __forceinline__ void tk_grid_sync(const tk_params &prm, unsigned target, unsigned) {
-    // One arrival per CTA.  (Per-warp arrivals -- 16 x 148 atomics on one address -- were measured: +1 us per barrier.)
+    // One arrival per CTA.  (Per-warp arrivals -- 16 atomics per CTA on one address -- make every barrier slower.)
     tk_bar_consumers(13);
     if (threadIdx.x == 0) {
         asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(prm.grid_bar) : "memory");
@@ -226,7 +226,7 @@ __device__ __forceinline__ void tk_load_ll(const float *base, int u, float v[E],
             v[2 * k + 1] = __uint_as_float(t[k].z);
         }
         if (ok) return;
-        // a failed round backs off: 148 CTAs x 512 threads spinning on the same words would otherwise keep the L2 busy with the polls
+        // a failed round backs off: every CTA's 512 threads spinning on the same words would otherwise keep the L2 busy with the polls
         // themselves -- and with it the stores they are waiting for and the weight stream
         __nanosleep(n < 4 ? 40u : 200u);
         if ((n & 255u) == 0) {                       // bounded like every other spin of this kernel
@@ -537,7 +537,7 @@ __device__ __forceinline__ void tk_consume(const tk_phase &ph, const tk_params &
             tk_slot_of(prm, g, idx, s, par);
             // A parity wait is only meaningful once the slot's PREVIOUS tile has completed its phase: the slots of a group are shared by
             // its four warps, so the previous tenant may be another warp's tile that has not even been issued yet -- and a parity wait
-            // answers "done" for a phase two ahead (seen on the B200 with shallow rings: garbage tiles, launch failures).  The producer
+            // answers "done" for a phase two ahead (seen with shallow rings: garbage tiles, launch failures).  The producer
             // tags the slot with the stream position once it owns it again (the previous tenant was consumed), then the wait is exact.
             tk_tag_wait(tags + s, idx + 1u, prm.err, 0x600u + (unsigned)warp, (unsigned)s);
             tk_mbar_wait(bar0 + 8u * s, par, prm.err, 0x400u + (unsigned)warp, (unsigned)s);
@@ -975,8 +975,7 @@ int flk_token_plan_create(const fl_token_step *steps, int n_steps, const uint16_
     tk_magic((uint32_t)p.Sg, p.s_magic, p.s_shift);
     p.slot_bytes = (uint32_t)slot;
     p.n_phases = n_steps;
-    // measured on B200 (round 1): prefetching a whole phase competes with the demand loads of the phase still running
-    // (7B decode 49.6 vs 45.8 us per layer), so it is opt-in
+    // prefetching a whole phase competes with the demand loads of the phase still running, so it is opt-in
     p.l2_prefetch = getenv("FASTLLAMA_B200_L2_PREFETCH") ? atoi(getenv("FASTLLAMA_B200_L2_PREFETCH")) : 0;
     p.exp_tab = exp_tab;
     p.diag = getenv("FASTLLAMA_B200_TK_DIAG") ? atoi(getenv("FASTLLAMA_B200_TK_DIAG")) : 0;
@@ -1033,7 +1032,7 @@ int flk_token_plan_launch(cudaStream_t st, void *plan) {
     fl_token_plan_impl *pl = (fl_token_plan_impl *)plan;
     FL_CUDA_OK(cudaMemsetAsync(pl->d_bar, 0, 4, st));
     void *args[] = {(void *)&pl->prm};
-    // cooperative launch: all 148 CTAs are guaranteed co-resident, which the grid barrier needs
+    // cooperative launch: all CTAs (one per SM) are guaranteed co-resident, which the grid barrier needs
     const void *fn = pl->prm.prof2 ? (const void *)k_decode_token<true> : (const void *)k_decode_token<false>;
     FL_CUDA_OK(cudaLaunchCooperativeKernel(fn, dim3(pl->n_kernels), dim3(TK_THREADS), args, pl->smem, st));
     fl_count_launch();

@@ -1,41 +1,37 @@
 // fl_umma_kernel.cu -- ggml_compute_forward_mul_mat_q_f32 for N > 1 (prompt ingest, n_batch = 128) on the
-// Blackwell tensor cores: tcgen05.mma kind::i8 with TMEM accumulators, weights fetched by TMA.
+// Hopper tensor cores: wgmma.mma_async with 8-bit integer operands, weights fetched by TMA.
 //
 // Reference semantics (lib/ggml.c:8105-8163 with ne11 = N, over :2445-2487 / :2639-2687):
 //     dst[n][m] = sum over 32-element blocks kb of
 //         d_w[m][kb] * d_y[n][kb] * ( sum_i (q4[m][kb][i] - 8) * q8[n][kb][i] )            (q4_0)
 //         d_w * d_y * sum_i q4 * q8  +  m_w[m][kb] * s_y[n][kb]                            (q4_1)
-// The per-block integer sum is exact in the reference and the scales are fp32.  ONE tcgen05.mma with
-// M = 128, N = NT, K = 32 (8-bit operands) is exactly one quant block for 128 weight rows x NT activation
-// columns, so the kernel issues one MMA per k-block into a fresh TMEM accumulator (no accumulation across
-// blocks on the tensor core), and the epilogue warps pull each s32 tile out of TMEM (tcgen05.ld) and do the
-// reference's fp32 step  acc = fma(d_w * d_y, float(isum), acc)  on the CUDA cores while the next MMAs run.
-// Accumulators rotate through the 512 TMEM columns in two groups of KG k-blocks (one synchronisation round per group).  Result: exactly the arithmetic of every other kernel of this
-// backend (exact block sums, fp32 scales, blocks added sequentially), so the same 2e-6 * sum|d q| budget.
+// The per-block integer sum is exact in the reference and the scales are fp32.  ONE wgmma with M = 64,
+// N = NT, K = 32 (8-bit operands) is exactly one quant block for 64 weight rows x NT activation columns, so
+// the kernel issues one MMA per k-block into a fresh register accumulator (scale-d = 0: no accumulation
+// across blocks on the tensor core) and the same warpgroup does the reference's fp32 step
+// acc = fma(d_w * d_y, float(isum), acc) on the CUDA cores.  Two accumulator sets alternate, so the MMA of
+// block kb + 1 runs while the epilogue of block kb does.  Result: exactly the arithmetic of every other kernel
+// of this backend (exact block sums, fp32 scales, blocks added sequentially), so the same 2e-6 * sum|d q| budget.
 //
-// Warp roles (448 threads, one CTA per 128-row x NT-column output tile):
-//   warps 0-3   unpack: thread r owns weight row r of the tile.  Raw q4 blocks (TMA tile [128 rows][KC blocks])
-//               -> 8-bit K-major operand in the canonical no-swizzle UMMA layout.  The k index inside a block is
-//               permuted to "16 low nibbles, then 16 high nibbles" (= even elements, then odd elements), the
-//               activations are stored in the same order, and integer sums do not care.  q4_0: bytes are (q - 8)
-//               as s8 (no correction term needed); q4_1: q as u8.  Also peels d (and m) into a per-row array.
-//   warps 4-11  epilogue: warp w reads TMEM lanes 32 * (w % 4) .. +31 (= rows), column half (w - 4) / 4.
-//   warp 12     TMA producer: weights by cp.async.bulk.tensor.2d (SASS UTMALDG), prepared activations and their
+// Roles (160 threads, one CTA per 64-row x NT-column output tile):
+//   warps 0-3   one consumer warpgroup.  Thread (warp w, lane 4g + t) builds its A fragment (rows 16w + g and
+//               16w + g + 8, k = 4t .. 4t + 3 and 16 + 4t .. 16 + 4t + 3) straight from ONE 32-bit word of each
+//               raw q4 block in shared memory: the k index inside a block is permuted to "16 low nibbles, then
+//               16 high nibbles" (= even elements, then odd elements), the activations are stored in the same
+//               order, and integer sums do not care.  q4_0: bytes are (q - 8) as s8; q4_1: q as u8.  B (the
+//               activations) is read by the tensor core from shared memory through a matrix descriptor.
+//   warp 4      TMA producer: weights by cp.async.bulk.tensor.2d (SASS UTMALDG), prepared activations and their
 //               scales by 1-D bulk copies, into a 4-stage mbarrier ring.
-//   warp 13     MMA issuer (one lane): tcgen05.mma + tcgen05.commit onto the mbarriers that free operands / publish
-//               accumulators.
 #include <cuda.h>
 #include <stdlib.h>
 
 #include "fl_common.cuh"
 #include "fl_kernels.h"
 
-#define UM_M 128
+#define UM_M 64               // weight rows per CTA = the M of one wgmma
 #define UM_KC 4               // k-blocks per TMA stage
 #define UM_STAGES 4
-#define UM_UNPACK_WARPS 4
-#define UM_EPI_WARPS 8
-#define UM_THREADS ((UM_UNPACK_WARPS + UM_EPI_WARPS + 2) * 32)
+#define UM_THREADS (4 * 32 + 32)
 
 // ---- PTX wrappers --------------------------------------------------------------------------------
 __device__ __forceinline__ void um_tma_2d(uint32_t dst, const CUtensorMap *tm, int c0, int c1, uint32_t bar) {
@@ -43,38 +39,62 @@ __device__ __forceinline__ void um_tma_2d(uint32_t dst, const CUtensorMap *tm, i
                  "r"(c1), "r"(bar)
                  : "memory");
 }
-__device__ __forceinline__ void um_fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void um_tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void um_tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void um_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] = A[smem] * B[smem], 8-bit integer operands, s32 accumulator, no accumulation into D (scale-d = 0)
-__device__ __forceinline__ void um_mma_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(0u), "r"(0u)
-        : "memory");
-}
-// K-major operand, no swizzle (cute::UMMA::SmemDescriptor): core matrix = 8 rows x 16 bytes, contiguous (128 B);
-// LBO = byte distance between the two 16-byte K halves, SBO = byte distance between 8-row groups; version 1 (sm_100)
+// K-major operand, no swizzle: core matrix = 8 rows x 16 bytes, contiguous (128 B); LBO = byte distance between the two
+// 16-byte K halves, SBO = byte distance between 8-row groups (wgmma matrix descriptor, swizzle mode 0)
 __device__ __forceinline__ uint64_t um_smem_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | ((uint64_t)1 << 46);
+    return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32);
 }
-#define UM_LD16(addr, v)                                                                                                                   \
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"   \
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), \
-                   "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])                                            \
-                 : "r"(addr)                                                                                                               \
-                 : "memory")
 // bounded mbarrier wait: a protocol bug traps (the launch fails with an error) instead of hanging the GPU
 __device__ __forceinline__ void um_wait(uint32_t bar, uint32_t parity) {
     for (uint32_t n = 0; !fl_mbar_try_wait(bar, parity); n++)
         if (n > (1u << 24)) asm volatile("trap;");
 }
-__device__ __forceinline__ void um_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void um_wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void um_wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void um_wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from touching accumulator registers while an MMA that writes them may be in flight
+template <int R>
+__device__ __forceinline__ void um_fence_regs(int32_t (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+r"(d[i])::"memory");
+}
+
+// D[regs] = A[regs] * B[smem], s32 accumulator, D not read (scale-d = 0).  A: s8 (q4_0, q - 8) or u8 (q4_1); B: s8.
+#define UM_R8(i) "+r"(d[i + 0]), "+r"(d[i + 1]), "+r"(d[i + 2]), "+r"(d[i + 3]), "+r"(d[i + 4]), "+r"(d[i + 5]), "+r"(d[i + 6]), "+r"(d[i + 7])
+template <int NT, bool A_S8>
+__device__ __forceinline__ void um_mma(int32_t (&d)[NT / 2], const uint32_t (&a)[4], uint64_t bdesc);
+template <>
+__device__ __forceinline__ void um_mma<32, true>(int32_t (&d)[16], const uint32_t (&a)[4], uint64_t bdesc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+                 "{%16, %17, %18, %19}, %20, p;\n\t}"
+                 : UM_R8(0), UM_R8(8)
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(0));
+}
+template <>
+__device__ __forceinline__ void um_mma<32, false>(int32_t (&d)[16], const uint32_t (&a)[4], uint64_t bdesc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k32.s32.u8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+                 "{%16, %17, %18, %19}, %20, p;\n\t}"
+                 : UM_R8(0), UM_R8(8)
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(0));
+}
+#define UM_D64 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}"
+template <>
+__device__ __forceinline__ void um_mma<64, true>(int32_t (&d)[32], const uint32_t (&a)[4], uint64_t bdesc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 " UM_D64 ", {%32, %33, %34, %35}, %36, p;\n\t}"
+                 : UM_R8(0), UM_R8(8), UM_R8(16), UM_R8(24)
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(0));
+}
+template <>
+__device__ __forceinline__ void um_mma<64, false>(int32_t (&d)[32], const uint32_t (&a)[4], uint64_t bdesc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k32.s32.u8.s8 " UM_D64 ", {%32, %33, %34, %35}, %36, p;\n\t}"
+                 : UM_R8(0), UM_R8(8), UM_R8(16), UM_R8(24)
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(0));
+}
 
 struct um_params {
     const uint8_t *yq;          // prepared activations: [ntiles][nbp][2][NT][16] bytes (even elements, odd elements)
@@ -83,33 +103,18 @@ struct um_params {
     size_t dst_row_stride;
     int M, N, nbp;              // nbp = k-blocks padded to a multiple of UM_KC
     int ntiles;                 // column tiles
-    int diag;                   // FASTLLAMA_B200_UMMA_DIAG (timing experiments only, results are garbage): 1 = no TMEM loads, 2 = no epilogue math
 };
 
-// Synchronisation is per GROUP of KG k-blocks (KG * NT = at most 256 TMEM columns; two groups in flight = all 512 columns):
-// one a_full / acc_full / acc_empty / a_empty round per group instead of per k-block.  Measured alternatives (7B, 128 tokens, all
-// matmuls): per-k-block rounds 16.0 ms; this 9.6 ms; deeper rings (8-12 operand tiles, 4 accumulator slots of 128 columns, row scales
-// travelling with the TMA stage) 14.0 - 14.4 ms -- every extra mbarrier operation costs the single MMA-issuing thread and the
-// epilogue warps ~100 cycles, which outweighs the extra slack.
 template <int TYPE, int NT>
 struct um_layout {
     static constexpr int BB = (TYPE == FL_TYPE_Q4_0) ? 20 : 24;
-    static constexpr int KG = (NT == 128) ? 2 : 4;                       // k-blocks per accumulator group
-    static constexpr int GPS = UM_KC / KG;                               // groups per TMA stage
-    static constexpr int RAW_A = UM_M * UM_KC * BB;                      // TMA box: 128 rows x KC blocks
+    static constexpr int RAW_A = UM_M * UM_KC * BB;                      // TMA box: 64 rows x KC blocks
     static constexpr int RAW_B = UM_KC * NT * 32;
     static constexpr int RAW_S = UM_KC * NT * 4;
     static constexpr int NSC = (TYPE == FL_TYPE_Q4_1) ? 2 : 1;           // scale arrays per stage (dy [, sy])
-    static constexpr int STAGE = RAW_A + RAW_B + NSC * RAW_S;
-    static constexpr int ATILE = UM_M * 32;                              // unpacked operand of one k-block
-    static constexpr int ASLOT = ATILE + NSC * UM_M * 4;                 // + d_w [, m_w] per row
-    static constexpr int AGROUP = KG * ASLOT;
-    static constexpr int OFF_A = UM_STAGES * STAGE;
-    static constexpr int OFF_BAR = OFF_A + 2 * AGROUP;
-    static constexpr int NBAR = 2 * UM_STAGES + 8;
-    static constexpr int SMEM = OFF_BAR + NBAR * 8 + 16;
-    static constexpr int CPT = NT / 2;                                   // columns per epilogue thread
-    static constexpr int TCOLS = 512;
+    static constexpr int STAGE = RAW_A + RAW_B + NSC * RAW_S;            // a multiple of 128 (TMA destinations)
+    static constexpr int OFF_BAR = UM_STAGES * STAGE;
+    static constexpr int SMEM = OFF_BAR + 2 * UM_STAGES * 8;
 };
 
 // ---- activations: q8_0 rows -> the operand layout of the MMA ------------------------------------------
@@ -147,242 +152,128 @@ __global__ void k_umma_prep(const fl_block_q8_0 *__restrict__ Y, int N, int nb, 
 }
 
 template <int TYPE, int NT>
-__global__ void __launch_bounds__(UM_THREADS, 1) k_mul_mat_q_umma(const __grid_constant__ CUtensorMap tmap_w, const um_params prm) {
+__global__ void __launch_bounds__(UM_THREADS) k_mul_mat_q_umma(const __grid_constant__ CUtensorMap tmap_w, const um_params prm) {
     using L = um_layout<TYPE, NT>;
-    constexpr int BB = L::BB, KG = L::KG, GPS = L::GPS;
+    constexpr int BB = L::BB, WPB = BB / 4, QOFF = WPB - 4;           // words per block, first qs word
+    constexpr int R = NT / 2;                                          // accumulator registers per thread
     extern __shared__ __align__(1024) uint8_t smem[];
-    __shared__ uint32_t tmem_base_sh;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile_n = blockIdx.x % prm.ntiles, tile_m = blockIdx.x / prm.ntiles;
     const int m0 = tile_m * UM_M, n0 = tile_n * NT;
-    const int nbp = prm.nbp, nstages = nbp / UM_KC;
+    const int nstages = prm.nbp / UM_KC;
 
     const uint32_t sm0 = fl_smem_u32(smem);
     const uint32_t bar0 = sm0 + L::OFF_BAR;
-    // barrier map (8 bytes each); g = accumulator / operand group slot (0, 1)
     auto raw_full = [&](int s) { return bar0 + 8u * s; };
     auto raw_empty = [&](int s) { return bar0 + 8u * (UM_STAGES + s); };
-    auto a_full = [&](int g) { return bar0 + 8u * (2 * UM_STAGES + g); };
-    auto a_empty = [&](int g) { return bar0 + 8u * (2 * UM_STAGES + 2 + g); };
-    auto acc_full = [&](int g) { return bar0 + 8u * (2 * UM_STAGES + 4 + g); };
-    auto acc_empty = [&](int g) { return bar0 + 8u * (2 * UM_STAGES + 6 + g); };
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < UM_STAGES; s++) {
             fl_mbar_init(raw_full(s), 1);
-            fl_mbar_init(raw_empty(s), UM_UNPACK_WARPS + UM_EPI_WARPS);     // the MMAs that read a stage's B tiles are complete before the epilogue lets go of it
-        }
-        for (int g = 0; g < 2; g++) {
-            fl_mbar_init(a_full(g), UM_UNPACK_WARPS);
-            fl_mbar_init(a_empty(g), UM_EPI_WARPS);                         // same: the epilogue has waited for the group's MMAs
-            fl_mbar_init(acc_full(g), 1);
-            fl_mbar_init(acc_empty(g), UM_EPI_WARPS);
+            fl_mbar_init(raw_empty(s), 4);                             // the four consumer warps, after their MMAs of the stage completed
         }
         fl_mbar_fence_init();
     }
-    if (warp == UM_UNPACK_WARPS + UM_EPI_WARPS + 1) {           // the MMA warp owns the TMEM allocation
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(fl_smem_u32(&tmem_base_sh)), "r"((uint32_t)L::TCOLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    um_tc_fence_before();
     __syncthreads();
-    um_tc_fence_after();
-    const uint32_t tmem_base = *(volatile uint32_t *)&tmem_base_sh;
 
-    if (warp < UM_UNPACK_WARPS) {
-        // ------------------------------------------------ unpack: raw q4 blocks -> 8-bit UMMA operand ---------------
-        const int r = threadIdx.x;                                // weight row of the tile
+    if (warp < 4) {
+        // ------------------------------------------------ consumer warpgroup: MMA + fp32 block scaling ------------
+        const int g = lane >> 2, t = lane & 3;
+        const int ra = 16 * warp + g, rb = ra + 8;                     // tile rows of this thread's A fragment and outputs
+        float acc[R], accm[(TYPE == FL_TYPE_Q4_1) ? R : 1];
+#pragma unroll
+        for (int j = 0; j < R; j++) acc[j] = 0.f;
+#pragma unroll
+        for (int j = 0; j < ((TYPE == FL_TYPE_Q4_1) ? R : 1); j++) accm[j] = 0.f;
+        int32_t d[2][R];
+#pragma unroll
+        for (int j = 0; j < R; j++) d[0][j] = d[1][j] = 0;
+
         for (int st = 0; st < nstages; st++) {
             const int s = st % UM_STAGES;
             um_wait(raw_full(s), (uint32_t)(st / UM_STAGES) & 1u);
-            // this row's KC blocks: 80 (q4_0) / 96 (q4_1) contiguous bytes, 16-byte aligned
-            uint32_t w[UM_KC * BB / 4];
-            const uint4 *src = (const uint4 *)(smem + (size_t)s * L::STAGE + (size_t)r * (UM_KC * BB));
+            const uint8_t *raw = smem + (size_t)s * L::STAGE;
+            const uint32_t *wa = (const uint32_t *)(raw + (size_t)ra * (UM_KC * BB));
+            const uint32_t *wb = (const uint32_t *)(raw + (size_t)rb * (UM_KC * BB));
+            const float *dys = (const float *)(raw + L::RAW_A + L::RAW_B);
+            const uint32_t bstage = sm0 + (uint32_t)(s * L::STAGE + L::RAW_A);
+            auto issue = [&](int i, int32_t(&dd)[R]) {
+                const uint32_t qa = wa[i * WPB + QOFF + t], qb = wb[i * WPB + QOFF + t];
+                uint32_t a[4] = {qa & 0x0F0F0F0Fu, qb & 0x0F0F0F0Fu, (qa >> 4) & 0x0F0F0F0Fu, (qb >> 4) & 0x0F0F0F0Fu};   // k 4t.. low, k 16 + 4t.. high nibbles
+                if (TYPE == FL_TYPE_Q4_0) {
 #pragma unroll
-            for (int i = 0; i < UM_KC * BB / 16; i++) {
-                const uint4 v = src[i];
-                w[4 * i] = v.x; w[4 * i + 1] = v.y; w[4 * i + 2] = v.z; w[4 * i + 3] = v.w;
+                    for (int j = 0; j < 4; j++) a[j] = (a[j] + 0x78787878u) ^ 0x80808080u;     // (x - 8) as s8, per byte, no carries
+                }
+                um_wg_fence();
+                um_mma<NT, TYPE == FL_TYPE_Q4_0>(dd, a, um_smem_desc(bstage + (uint32_t)(i * NT * 32), NT * 16, 128));
+                um_wg_commit();
+            };
+            issue(0, d[0]);
+#pragma unroll
+            for (int i = 0; i < UM_KC; i++) {
+                if (i + 1 < UM_KC) {
+                    issue(i + 1, d[(i + 1) & 1]);
+                    um_wg_wait<1>();
+                } else {
+                    um_wg_wait<0>();
+                }
+                int32_t(&v)[R] = d[i & 1];
+                um_fence_regs(v);
+                // outputs of register 4j + e: row (e < 2 ? ra : rb), column 8j + 2t + (e & 1)
+                const float dwa = __uint_as_float(wa[i * WPB]), dwb = __uint_as_float(wb[i * WPB]);
+                const float *dyi = dys + i * NT;
+#pragma unroll
+                for (int j = 0; j < NT / 8; j++) {
+                    const float2 y = *(const float2 *)(dyi + 8 * j + 2 * t);
+                    acc[4 * j + 0] = __fmaf_rn(__fmul_rn(dwa, y.x), __int2float_rn(v[4 * j + 0]), acc[4 * j + 0]);
+                    acc[4 * j + 1] = __fmaf_rn(__fmul_rn(dwa, y.y), __int2float_rn(v[4 * j + 1]), acc[4 * j + 1]);
+                    acc[4 * j + 2] = __fmaf_rn(__fmul_rn(dwb, y.x), __int2float_rn(v[4 * j + 2]), acc[4 * j + 2]);
+                    acc[4 * j + 3] = __fmaf_rn(__fmul_rn(dwb, y.y), __int2float_rn(v[4 * j + 3]), acc[4 * j + 3]);
+                }
+                if (TYPE == FL_TYPE_Q4_1) {
+                    const float mwa = __uint_as_float(wa[i * WPB + 1]), mwb = __uint_as_float(wb[i * WPB + 1]);
+                    const float *syi = dyi + UM_KC * NT;
+#pragma unroll
+                    for (int j = 0; j < NT / 8; j++) {
+                        const float2 y = *(const float2 *)(syi + 8 * j + 2 * t);
+                        accm[4 * j + 0] = __fmaf_rn(mwa, y.x, accm[4 * j + 0]);
+                        accm[4 * j + 1] = __fmaf_rn(mwa, y.y, accm[4 * j + 1]);
+                        accm[4 * j + 2] = __fmaf_rn(mwb, y.x, accm[4 * j + 2]);
+                        accm[4 * j + 3] = __fmaf_rn(mwb, y.y, accm[4 * j + 3]);
+                    }
+                }
             }
             __syncwarp();
-            if (lane == 0) fl_mbar_arrive(raw_empty(s));          // the raw weights of this stage are in registers
+            if (lane == 0) fl_mbar_arrive(raw_empty(s));               // every MMA reading this stage has completed (wait_group 0)
+        }
+        // store: column n of the output is M contiguous floats
 #pragma unroll
-            for (int gs = 0; gs < GPS; gs++) {
-                const int gi = st * GPS + gs;                      // group index; slot gi & 1, use gi >> 1
-                const int g = gi & 1;
-                um_wait(a_empty(g), ((uint32_t)(gi >> 1) & 1u) ^ 1u);
-#pragma unroll
-                for (int i = 0; i < KG; i++) {
-                    const int kbi = gs * KG + i;
-                    uint8_t *slot = smem + L::OFF_A + (size_t)g * L::AGROUP + (size_t)i * L::ASLOT;
-                    constexpr int WPB = BB / 4;                    // words per block
-                    constexpr int QOFF = WPB - 4;                  // first qs word
-                    uint32_t lo[4], hi[4];
-#pragma unroll
-                    for (int j = 0; j < 4; j++) {
-                        const uint32_t q = w[kbi * WPB + QOFF + j];
-                        lo[j] = q & 0x0F0F0F0Fu;
-                        hi[j] = (q >> 4) & 0x0F0F0F0Fu;
-                        if (TYPE == FL_TYPE_Q4_0) {                // (x - 8) as s8, per byte, no carries: (x + 0x78) ^ 0x80
-                            lo[j] = (lo[j] + 0x78787878u) ^ 0x80808080u;
-                            hi[j] = (hi[j] + 0x78787878u) ^ 0x80808080u;
-                        }
-                    }
-                    *(uint4 *)(slot + (size_t)r * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);                 // k = 0..15: low nibbles = even elements
-                    *(uint4 *)(slot + (size_t)UM_M * 16 + (size_t)r * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);   // k = 16..31: high nibbles = odd elements
-                    float *dw = (float *)(slot + L::ATILE);
-                    dw[r] = __uint_as_float(w[kbi * WPB]);
-                    if (TYPE == FL_TYPE_Q4_1) dw[UM_M + r] = __uint_as_float(w[kbi * WPB + 1]);
-                }
-                um_fence_proxy_async();                            // generic-proxy stores -> visible to the tensor core's async proxy
-                __syncwarp();
-                if (lane == 0) fl_mbar_arrive(a_full(g));
+        for (int j = 0; j < R; j++) {
+            const int row = m0 + (((j >> 1) & 1) ? rb : ra);
+            const int col = n0 + 8 * (j >> 2) + 2 * t + (j & 1);
+            if (row < prm.M && col < prm.N) {
+                float o = acc[j];
+                if (TYPE == FL_TYPE_Q4_1) o = __fadd_rn(acc[j], accm[j]);
+                prm.dst[(size_t)col * prm.dst_row_stride + (size_t)row] = o;
             }
         }
-    } else if (warp < UM_UNPACK_WARPS + UM_EPI_WARPS) {
-        // ------------------------------------------------ epilogue: TMEM -> fp32 block scaling -> registers ----------
-        const int ew = warp - UM_UNPACK_WARPS;
-        const int quad = warp & 3;                                 // TMEM lanes 32 * quad .. + 31 are the ones this warp may touch
-        const int half = ew >> 2;
-        constexpr int CPT = L::CPT;
-        constexpr int CW = CPT < 32 ? CPT : 32;                    // columns per TMEM round trip (keeps v[] at 32 registers)
-        const int row = quad * 32 + lane;
-        const int c0 = half * CPT;
-        float2 acc[CPT / 2], accm[(TYPE == FL_TYPE_Q4_1) ? CPT / 2 : 1];
-#pragma unroll
-        for (int j = 0; j < CPT / 2; j++) acc[j] = make_float2(0.f, 0.f);
-#pragma unroll
-        for (int j = 0; j < ((TYPE == FL_TYPE_Q4_1) ? CPT / 2 : 1); j++) accm[j] = make_float2(0.f, 0.f);
+    } else if (lane == 0) {
+        // ------------------------------------------------ TMA producer ------------------------------------------------
+        const int nbp = prm.nbp;
+        const uint8_t *yq = prm.yq + (size_t)tile_n * nbp * (size_t)(NT * 32);
+        const float *dy = prm.dy + (size_t)tile_n * nbp * NT;
+        const float *sy = prm.sy + (size_t)tile_n * nbp * NT;
         for (int st = 0; st < nstages; st++) {
             const int s = st % UM_STAGES;
-            um_wait(raw_full(s), (uint32_t)(st / UM_STAGES) & 1u);          // the stage's d_y / s_y have landed
-            const float *dys = (const float *)(smem + (size_t)s * L::STAGE + L::RAW_A + L::RAW_B);
-#pragma unroll 1
-            for (int gs = 0; gs < GPS; gs++) {
-                const int gi = st * GPS + gs;
-                const int g = gi & 1;
-                const uint32_t par = (uint32_t)(gi >> 1) & 1u;
-                um_wait(a_full(g), par);                           // acquire the unpack warps' d_w stores
-                um_wait(acc_full(g), par);
-                um_tc_fence_after();
-#pragma unroll
-                for (int i = 0; i < KG; i++) {
-                    const int kbi = gs * KG + i;
-                    const float *dwp = (const float *)(smem + L::OFF_A + (size_t)g * L::AGROUP + (size_t)i * L::ASLOT + L::ATILE);
-                    const float dwm = dwp[row];
-                    const float2 dw2 = make_float2(dwm, dwm);
-                    const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(g * 256 + i * NT + c0);
-#pragma unroll
-                    for (int ch = 0; ch < CPT / CW; ch++) {
-                        uint32_t v[CW];
-                        if (prm.diag & 1) {
-#pragma unroll
-                            for (int c = 0; c < CW; c++) v[c] = (uint32_t)(c + kbi);
-                        } else {
-#pragma unroll
-                            for (int c = 0; c < CW / 16; c++) UM_LD16(taddr + (uint32_t)(ch * CW + 16 * c), (&v[16 * c]));
-                            um_wait_ld();
-                        }
-                        if (i == KG - 1 && ch == CPT / CW - 1) {   // every column of the group's accumulators is in registers: hand them back
-                            um_tc_fence_before();
-                            __syncwarp();
-                            if (lane == 0) fl_mbar_arrive(acc_empty(g));
-                        }
-                        const float4 *dy4 = (const float4 *)(dys + kbi * NT + c0 + ch * CW);
-                        if (prm.diag & 2) { if (v[0] == 0x7fffffffu) acc[0].x += 1.f; continue; }
-#pragma unroll
-                        for (int j = 0; j < CW / 4; j++) {
-                            const float4 d4 = dy4[j];
-                            // packed fp32 (FMUL2 / FFMA2): element-wise IEEE round-to-nearest, the same results as the scalar forms
-                            const float2 s01 = __fmul2_rn(dw2, make_float2(d4.x, d4.y)), s23 = __fmul2_rn(dw2, make_float2(d4.z, d4.w));
-                            const float2 i01 = make_float2(__int2float_rn((int)v[4 * j + 0]), __int2float_rn((int)v[4 * j + 1]));
-                            const float2 i23 = make_float2(__int2float_rn((int)v[4 * j + 2]), __int2float_rn((int)v[4 * j + 3]));
-                            float2 *a = acc + (ch * CW + 4 * j) / 2;
-                            a[0] = __ffma2_rn(s01, i01, a[0]);
-                            a[1] = __ffma2_rn(s23, i23, a[1]);
-                        }
-                    }
-                    if (TYPE == FL_TYPE_Q4_1) {
-                        const float mwm = dwp[UM_M + row];
-                        const float2 mw2 = make_float2(mwm, mwm);
-                        const float4 *sy4 = (const float4 *)(dys + UM_KC * NT + kbi * NT + c0);
-#pragma unroll
-                        for (int j = 0; j < CPT / 4; j++) {
-                            const float4 s4 = sy4[j];
-                            accm[2 * j] = __ffma2_rn(mw2, make_float2(s4.x, s4.y), accm[2 * j]);
-                            accm[2 * j + 1] = __ffma2_rn(mw2, make_float2(s4.z, s4.w), accm[2 * j + 1]);
-                        }
-                    }
-                }
-                __syncwarp();
-                if (lane == 0) fl_mbar_arrive(a_empty(g));         // d_w / m_w of the group have been read (and its MMAs are long complete)
-            }
-            __syncwarp();
-            if (lane == 0) fl_mbar_arrive(raw_empty(s));           // d_y / s_y of the stage have been read
+            um_wait(raw_empty(s), ((uint32_t)(st / UM_STAGES) & 1u) ^ 1u);
+            const uint32_t dst = sm0 + (uint32_t)(s * L::STAGE);
+            const int kb0 = st * UM_KC;
+            fl_mbar_expect_tx(raw_full(s), (uint32_t)L::STAGE);
+            um_tma_2d(dst, &tmap_w, kb0 * (BB / 4), m0, raw_full(s));                                   // 64 rows x KC blocks of raw q4
+            fl_bulk_g2s(dst + L::RAW_A, yq + (size_t)kb0 * (NT * 32), (uint32_t)L::RAW_B, raw_full(s));
+            fl_bulk_g2s(dst + L::RAW_A + L::RAW_B, dy + (size_t)kb0 * NT, (uint32_t)L::RAW_S, raw_full(s));
+            if (TYPE == FL_TYPE_Q4_1) fl_bulk_g2s(dst + L::RAW_A + L::RAW_B + L::RAW_S, sy + (size_t)kb0 * NT, (uint32_t)L::RAW_S, raw_full(s));
         }
-        // store: column n of the output is M contiguous floats; a warp writes 32 consecutive rows of one column
-        if (m0 + row < prm.M) {
-#pragma unroll
-            for (int j = 0; j < CPT; j++) {
-                const int col = n0 + c0 + j;
-                if (col < prm.N) {
-                    const float a = (j & 1) ? acc[j / 2].y : acc[j / 2].x;
-                    float o = a;
-                    if (TYPE == FL_TYPE_Q4_1) o = __fadd_rn(a, (j & 1) ? accm[j / 2].y : accm[j / 2].x);
-                    prm.dst[(size_t)col * prm.dst_row_stride + (size_t)(m0 + row)] = o;
-                }
-            }
-        }
-    } else if (warp == UM_UNPACK_WARPS + UM_EPI_WARPS) {
-        // ------------------------------------------------ TMA producer ------------------------------------------------
-        if (lane == 0) {
-            const uint8_t *yq = prm.yq + (size_t)tile_n * nbp * (size_t)(NT * 32);
-            const float *dy = prm.dy + (size_t)tile_n * nbp * NT;
-            const float *sy = prm.sy + (size_t)tile_n * nbp * NT;
-            for (int st = 0; st < nstages; st++) {
-                const int s = st % UM_STAGES;
-                um_wait(raw_empty(s), ((uint32_t)(st / UM_STAGES) & 1u) ^ 1u);
-                const uint32_t dst = sm0 + (uint32_t)(s * L::STAGE);
-                const int kb0 = st * UM_KC;
-                fl_mbar_expect_tx(raw_full(s), (uint32_t)L::STAGE);
-                um_tma_2d(dst, &tmap_w, kb0 * (BB / 4), m0, raw_full(s));                                   // 128 rows x KC blocks of raw q4
-                fl_bulk_g2s(dst + L::RAW_A, yq + (size_t)kb0 * (NT * 32), (uint32_t)L::RAW_B, raw_full(s));
-                fl_bulk_g2s(dst + L::RAW_A + L::RAW_B, dy + (size_t)kb0 * NT, (uint32_t)L::RAW_S, raw_full(s));
-                if (TYPE == FL_TYPE_Q4_1) fl_bulk_g2s(dst + L::RAW_A + L::RAW_B + L::RAW_S, sy + (size_t)kb0 * NT, (uint32_t)L::RAW_S, raw_full(s));
-            }
-        }
-    } else {
-        // ------------------------------------------------ MMA issuer ----------------------------------------------------
-        if (lane == 0) {
-            // instruction descriptor (cute::UMMA::InstrDescriptor): D = s32, A = s8 (q4_0: q - 8) / u8 (q4_1), B = s8, both K-major
-            constexpr uint32_t idesc = (2u << 4) | ((TYPE == FL_TYPE_Q4_0 ? 1u : 0u) << 7) | (1u << 10) | ((uint32_t)(NT >> 3) << 17) | ((uint32_t)(UM_M >> 4) << 24);
-            for (int st = 0; st < nstages; st++) {
-                const int s = st % UM_STAGES;
-                um_wait(raw_full(s), (uint32_t)(st / UM_STAGES) & 1u);
-                const uint32_t bstage = sm0 + (uint32_t)(s * L::STAGE + L::RAW_A);
-                for (int gs = 0; gs < GPS; gs++) {
-                    const int gi = st * GPS + gs;
-                    const int g = gi & 1;
-                    const uint32_t par = (uint32_t)(gi >> 1) & 1u;
-                    um_wait(a_full(g), par);
-                    um_wait(acc_empty(g), par ^ 1u);
-                    um_tc_fence_after();
-#pragma unroll
-                    for (int i = 0; i < KG; i++) {
-                        const int kbi = gs * KG + i;
-                        const uint64_t adesc = um_smem_desc(sm0 + (uint32_t)(L::OFF_A + g * L::AGROUP + i * L::ASLOT), UM_M * 16, 128);
-                        const uint64_t bdesc = um_smem_desc(bstage + (uint32_t)(kbi * NT * 32), NT * 16, 128);
-                        um_mma_i8(tmem_base + (uint32_t)(g * 256 + i * NT), adesc, bdesc, idesc);
-                    }
-                    um_commit(acc_full(g));                        // arrives when the group's MMAs (and everything before them) are complete
-                }
-            }
-        }
-    }
-    um_tc_fence_before();
-    __syncthreads();
-    if (warp == UM_UNPACK_WARPS + UM_EPI_WARPS + 1) {
-        um_tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)L::TCOLS) : "memory");
     }
 }
 
@@ -434,14 +325,13 @@ static int um_launch(cudaStream_t st, const void *W, size_t wrs, int M, int K, c
     const cuuint32_t estr[2] = {1, 1};
     const CUresult cr = um_get_encode()(&tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, (void *)W, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                         CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    FL_REQUIRE(cr == CUDA_SUCCESS, "mul_mat_q (tcgen05): cuTensorMapEncodeTiled failed (%d) for M=%d K=%d stride=%zu", (int)cr, M, K, wrs);
+    FL_REQUIRE(cr == CUDA_SUCCESS, "mul_mat_q (wgmma): cuTensorMapEncodeTiled failed (%d) for M=%d K=%d stride=%zu", (int)cr, M, K, wrs);
     static bool attr_done = false;
     if (!attr_done) {
         FL_CUDA_OK(cudaFuncSetAttribute(k_mul_mat_q_umma<TYPE, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM));
         attr_done = true;
     }
     um_params p;
-    p.diag = getenv("FASTLLAMA_B200_UMMA_DIAG") ? atoi(getenv("FASTLLAMA_B200_UMMA_DIAG")) : 0;
     p.yq = g_um.yq; p.dy = g_um.dy; p.sy = g_um.sy; p.dst = dst; p.dst_row_stride = drs; p.M = M; p.N = N; p.nbp = nbp; p.ntiles = ntiles;
     k_mul_mat_q_umma<TYPE, NT><<<mtiles * ntiles, UM_THREADS, L::SMEM, st>>>(tm, p);
     fl_count_launch();
@@ -449,24 +339,20 @@ static int um_launch(cudaStream_t st, const void *W, size_t wrs, int M, int K, c
     return 0;
 }
 
-// nt_hint: 0 = choose, else 32 / 64 / 128 (q4_1: at most 64, the epilogue keeps two accumulators per output)
+// nt_hint: 0 = choose, else 32 / 64 (128 is taken as 64: two register accumulator sets of 64 columns are the most a
+// warpgroup keeps beside its fp32 sums without spilling)
 int flk_mul_mat_q_umma(cudaStream_t st, int type, const void *W, size_t wrs, int M, int K, const void *Yq8, int N, float *dst, size_t drs, int nt_hint) {
-    FL_REQUIRE(flk_mul_mat_q_umma_supported(type, W, wrs, M, K, N), "mul_mat_q (tcgen05): unsupported operands (type %d, W %p, stride %zu, K %d)", type, W, wrs, K);
+    FL_REQUIRE(flk_mul_mat_q_umma_supported(type, W, wrs, M, K, N), "mul_mat_q (wgmma): unsupported operands (type %d, W %p, stride %zu, K %d)", type, W, wrs, K);
     int nt = nt_hint;
     if (nt == 0) {
-        // enough CTAs to cover the SMs: prefer wide column tiles (weights are re-read once per column tile)
-        const int mtiles = (M + UM_M - 1) / UM_M, sms = flk_sm_count();
-        nt = 32;
-        for (int c = 128; c >= 64; c /= 2)
-            if (N > c / 2 && mtiles * ((N + c - 1) / c) >= sms - sms / 8) { nt = c; break; }
-        if (N > 32 && nt == 32 && mtiles * ((N + 63) / 64) >= sms / 2) nt = 64;
+        // wide column tiles re-read the weights less often; narrow ones when the wide tiling leaves SMs idle
+        const int mtiles = (M + UM_M - 1) / UM_M;
+        nt = (N > 32 && mtiles * ((N + 63) / 64) >= flk_sm_count()) ? 64 : 32;
     }
-    if (type == FL_TYPE_Q4_1 && nt > 64) nt = 64;
-    if (type == FL_TYPE_Q4_0) {
-        if (nt == 128) return um_launch<FL_TYPE_Q4_0, 128>(st, W, wrs, M, K, Yq8, N, dst, drs);
-        if (nt == 64) return um_launch<FL_TYPE_Q4_0, 64>(st, W, wrs, M, K, Yq8, N, dst, drs);
-        return um_launch<FL_TYPE_Q4_0, 32>(st, W, wrs, M, K, Yq8, N, dst, drs);
+    if (nt >= 64) {
+        if (type == FL_TYPE_Q4_0) return um_launch<FL_TYPE_Q4_0, 64>(st, W, wrs, M, K, Yq8, N, dst, drs);
+        return um_launch<FL_TYPE_Q4_1, 64>(st, W, wrs, M, K, Yq8, N, dst, drs);
     }
-    if (nt == 64) return um_launch<FL_TYPE_Q4_1, 64>(st, W, wrs, M, K, Yq8, N, dst, drs);
+    if (type == FL_TYPE_Q4_0) return um_launch<FL_TYPE_Q4_0, 32>(st, W, wrs, M, K, Yq8, N, dst, drs);
     return um_launch<FL_TYPE_Q4_1, 32>(st, W, wrs, M, K, Yq8, N, dst, drs);
 }

@@ -1,5 +1,5 @@
 // ggml_b200.cpp -- ggml-compatible host library (boundary B1, include/fl_ggml.h) whose
-// ggml_graph_compute runs on a B200 through the extern-"C" CUDA layer (include/fl_cuda.h).
+// ggml_graph_compute runs on an H100 through the extern-"C" CUDA layer (include/fl_cuda.h).
 //
 // Plain host C++ (compiled by g++, no CUDA headers).  Three parts:
 //   1. tensor arena + graph builders: same observable behaviour and space accounting as the
@@ -656,6 +656,49 @@ static void drop_external_mirrors() {
     if (any) packed_shards_clear();
     g_last_mirror = -1;
 }
+// [lo, hi) of the process's anonymous (not file-backed) memory mappings, in address order
+static std::vector<std::pair<uintptr_t, uintptr_t>> anon_mappings() {
+    std::vector<std::pair<uintptr_t, uintptr_t>> r;
+    FILE *f = fopen("/proc/self/maps", "r");
+    if (!f) return r;
+    char line[4096];
+    while (fgets(line, sizeof line, f)) {
+        unsigned long lo, hi, off, inode;
+        unsigned dmaj, dmin;
+        char perms[8];
+        if (sscanf(line, "%lx-%lx %7s %lx %x:%x %lu", &lo, &hi, perms, &off, &dmaj, &dmin, &inode) == 7 && inode == 0) r.push_back({lo, hi});
+    }
+    fclose(f);
+    return r;
+}
+static bool anon_mapped(const std::vector<std::pair<uintptr_t, uintptr_t>> &maps, const char *p, size_t n) {
+    uintptr_t a = (uintptr_t)p;
+    const uintptr_t e = a + n;
+    for (const auto &m : maps) {
+        if (m.second <= a) continue;
+        if (m.first > a) return false;
+        a = m.second;
+        if (a >= e) return true;
+    }
+    return false;
+}
+// Arena and scratch buffers are heap memory.  One that is no longer (wholly) backed by anonymous memory has been freed and unmapped,
+// and a new mapping -- the next model's weights -- may lie on its addresses: its record would be taken for the new tensors and
+// serve the old buffer's device copy.  Such records are dropped when a model is loaded; live buffers keep theirs.
+static void drop_unmapped_arenas() {
+    const auto maps = anon_mappings();
+    if (maps.empty()) return;
+    bool any = false;
+    for (auto &m : g_mirrors) {
+        if (!m.alive || m.kind == MK_EXTERNAL || anon_mapped(maps, m.host, m.size)) continue;
+        if (!any && fl_is_initialized()) fl_sync();
+        any = true;
+        drop_mirror(m);
+        m.alive = false;
+        m.uploaded = 0;
+    }
+    g_last_mirror = -1;
+}
 static void mirrors_on_ctx_init(ggml_context *ctx) {
     // an arena re-created over the same buffer (Model::eval does this every call) re-uses its mirror
     int found = -1;
@@ -677,7 +720,10 @@ static void mirrors_on_ctx_init(ggml_context *ctx) {
     // (include/tensor/mem_context.hpp:12-16, lib/llama.cpp:213-258).  MK_EXTERNAL mirrors are keyed by host address only, and a
     // new mapping may land on the addresses of an earlier model's: everything registered for earlier mappings is stale now.
     // (A model that is still alive simply re-registers and re-uploads its tensors on next use.)
-    if (ctx->no_alloc) drop_external_mirrors();
+    if (ctx->no_alloc) {
+        drop_external_mirrors();
+        drop_unmapped_arenas();
+    }
 }
 static void mirrors_on_ctx_free(ggml_context *) {}   // the arena (and its device mirror) outlives the context slot
 static void mirrors_note_alloc(ggml_context *ctx, size_t end) {
@@ -777,11 +823,12 @@ extern "C" void ggml_b200_release_all(void) {
     for (auto &m : g_mirrors) {
         drop_mirror(m);
         m.uploaded = 0;
-        if (m.device_dirty) { m.device_dirty = false; g_dirty_arenas.fetch_sub(1, std::memory_order_release); }
-        if (m.kind != MK_ARENA) m.alive = false;
+        m.alive = false;
     }
-    // arenas whose host buffer is gone would never be matched again: forget all records (a live arena re-registers at its next ggml_init,
-    // and a context that is still open keeps working because mirror lookups are by address)
+    // Forget all records, arenas included: the closed model's buffers are freed, and a later mapping (the next model's weights) may
+    // land on their addresses; a record left alive there would be taken for the new tensors and upload from the old, now unmapped,
+    // range.  A live arena re-registers at its next ggml_init, and a context that is still open keeps working because mirror lookups
+    // are by address.
     g_last_mirror = -1;
 }
 // how the last single-token eval ran: 0 = node-by-node executor, 1 = fused plan with one kernel per matrix group,

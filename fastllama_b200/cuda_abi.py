@@ -132,7 +132,7 @@ SIGNATURES = {
 
 
 class FlCuda:
-    """Loaded libfl_cuda.so.  ``FlCuda(init=True)`` needs a B200."""
+    """Loaded libfl_cuda.so.  ``FlCuda(init=True)`` needs an H100."""
 
     def __init__(self, path: str | None = None, init: bool = True, device: int = -1):
         path = path or lib_path("libfl_cuda.so")

@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's Python API (reference interfaces/python/fastllama.py:194-479)
 over the same C ABI (reference interfaces/c/fastllama.h), so a user of ``fastllama.Model`` can switch by
 changing the import.  By default it loads the drop-in ``pyfastllama.so`` of this repository (the
-reference's unchanged bridge over the B200 backend); ``library_path`` may point at any library that
+reference's unchanged bridge over the H100 backend); ``library_path`` may point at any library that
 exports the same 17 ``llama_*`` symbols -- the tests pass the reference build to get the CPU oracle.
 
 Same names, argument meaning and error behaviour as the reference: ``bool`` returns, RuntimeError when

@@ -1,5 +1,5 @@
 /*
- * fl_cuda.h -- the thin extern-"C" CUDA layer of the B200 backend (libfl_cuda.so).
+ * fl_cuda.h -- the thin extern-"C" CUDA layer of the H100 backend (libfl_cuda.so).
  *
  * Plain pointers and sizes only; no C++ or torch types cross this boundary.  Every entry point
  * cites the reference interface it replaces (file:line relative to the reference tree).
@@ -8,7 +8,7 @@
  *   (1) HOST-BUFFER entry points: drop-in replacements for the row functions the reference
  *       dispatches through quantize_fns[type] (lib/ggml.c:1731-1773, type quantize_fns_t
  *       include/ggml.h:850-862) and for ggml_compute_forward_mul_mat_q_f32.  Inputs and outputs
- *       are host memory; each call does H2D -> sm_100a kernel -> D2H on the library stream and
+ *       are host memory; each call does H2D -> sm_90a kernel -> D2H on the library stream and
  *       returns when the result is in the output buffer.  This is what a cgo/ctypes/FFI binding of
  *       the reference's test hook (ggml_internal_get_quantize_fn) would bind.
  *   (2) DEVICE-RESIDENT entry points (fl_dev_*): the same kernels on device pointers, used by the
@@ -92,11 +92,11 @@ int fl_host_free_pinned(void *p);
 /* activations -> q8_0 rows.  x row r starts at x + r*x_row_stride_bytes; y rows are packed. */
 int fl_dev_quantize_q8_0(const float *x, size_t x_row_stride_bytes, void *y, int k, int nrows);
 
-/* dst[n*dst_row_stride + m] = vec_dot(W row m, Yq8 row n).  impl: 0 = auto (N = 1: ring; N >= 16: tcgen05 GEMM; N >= 4: mma.sync kernel;
+/* dst[n*dst_row_stride + m] = vec_dot(W row m, Yq8 row n).  impl: 0 = auto (N = 1: ring; N >= 16: wgmma GEMM; N >= 4: mma.sync kernel;
  * else plain), 1 = plain warp-per-row LDG kernel, 2 = TMA-bulk-staged persistent matvec (N = 1 only), 3 = legacy tensor-core kernel
- * (mma.sync m16n8k32 u8 x s8 block sums, fp32 scales; any N), 4 = tcgen05 GEMM (fl_umma_kernel.cu: one tcgen05.mma kind::i8 M = 128,
- * K = 32 per quant block into TMEM, weights by TMA, exact fp32 block scaling in the epilogue; needs 16-byte aligned W rows), 5 / 6 / 7 = the
- * same with the column tile forced to 32 / 64 / 128 (7: q4_0 only). */
+ * (mma.sync m16n8k32 u8 x s8 block sums, fp32 scales; any N), 4 = wgmma GEMM (fl_umma_kernel.cu: one wgmma M = 64,
+ * K = 32 with 8-bit operands per quant block into registers, weights by TMA, exact fp32 block scaling; needs 16-byte aligned W rows),
+ * 5 / 6 / 7 = the same with the column tile forced to 32 / 64 / 64. */
 int fl_dev_mul_mat_q(int type, const void *W, size_t w_row_stride_bytes, int M, int K, const void *Yq8, int N,
                      float *dst, size_t dst_row_stride_elems, int impl);
 

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def _have_gpu() -> bool:
@@ -22,12 +22,12 @@ def _have_gpu() -> bool:
 
 
 def pytest_collection_modifyitems(config, items):
-    """A plain `pytest tests` on a box without a CUDA device skips the gpu-marked tests.  With `-m gpu` (the B200 run) or
+    """A plain `pytest tests` on a box without a CUDA device skips the gpu-marked tests.  With `-m gpu` (the H100 run) or
     FASTLLAMA_B200_STRICT_GPU=1 nothing is skipped: a missing device or library must FAIL there, never pass silently."""
     strict = os.environ.get("FASTLLAMA_B200_STRICT_GPU") == "1" or "gpu" in (config.getoption("-m") or "").replace("not gpu", "")
     if strict or _have_gpu():
         return
-    skip = pytest.mark.skip(reason="no CUDA device (gpu tests run on the B200 box; set FASTLLAMA_B200_STRICT_GPU=1 to force)")
+    skip = pytest.mark.skip(reason="no CUDA device (gpu tests run on an H100; set FASTLLAMA_B200_STRICT_GPU=1 to force)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

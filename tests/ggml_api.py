@@ -1,5 +1,5 @@
 """ctypes driver for the ggml C API -- the SAME script drives the reference (oracle/_ref/libggml_ref.so,
-CPU) and our drop-in (fastllama_b200/lib/libggml_b200.so, B200), which is the point of boundary B1.
+CPU) and our drop-in (fastllama_b200/lib/libggml_b200.so, H100), which is the point of boundary B1.
 
 Struct layouts: reference include/ggml.h:267-342 (mirrored in include/fl_ggml.h).
 """

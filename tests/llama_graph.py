@@ -1,6 +1,6 @@
 """The LLaMA eval graph, built through the ggml C API exactly as the reference's Model::eval builds it
 (reference lib/llama.cpp:297-474), so the same script can run on the reference library (CPU) and on
-libggml_b200 (B200) and every node can be compared.  Three arenas like the reference: weights
+libggml_b200 (H100) and every node can be compared.  Three arenas like the reference: weights
 (Model::ctx), KV cache (kv_self.ctx), compute (buf_compute, re-initialised per eval).
 """
 from __future__ import annotations

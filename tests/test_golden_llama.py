@@ -5,7 +5,7 @@ a tiny LLaMA built through the ggml C API like Model::eval builds it, 5-token pr
   * CPU: our host stack (arena mirrors, executor, decode plan as the token program) on the CPU stand-in of the device layer;
   * GPU: the real thing -- prompt through the tensor-core ingest kernel, decode steps as the persistent token kernel.
 Bar for ours: the SAME BITS as the reference library, logits and embeddings, prompt eval and decode steps (every fp32 operation of the
-path follows the reference's order, fl_exact.cuh; the 5-token prompt stays below the 16 columns from which the tcgen05 GEMM takes over)."""
+path follows the reference's order, fl_exact.cuh; the 5-token prompt stays below the 16 columns from which the wgmma GEMM takes over)."""
 import os
 
 import numpy as np

@@ -5,7 +5,7 @@ via the same Python Model class (fastllama_b200/model.py, mirror of the referenc
 
 north_star bar: greedy token-id sequence identical; logits within a stated fp tolerance.  The tolerance here is ZERO: the logits after
 the prompt and the decode steps carry the reference's bits (every fp32 operation in the reference's order, fl_exact.cuh; the prompt of
-these tests stays below the 16 columns from which the tcgen05 GEMM -- reordering budget, not bit-identical -- takes over).
+these tests stays below the 16 columns from which the wgmma GEMM -- reordering budget, not bit-identical -- takes over).
 """
 import os
 

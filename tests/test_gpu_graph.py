@@ -1,5 +1,5 @@
 """GPU: boundary B1 end to end.  The same ggml-API script runs on the reference library (CPU,
-oracle/_ref/libggml_ref.so) and on libggml_b200 (B200); results are compared op by op and for whole
+oracle/_ref/libggml_ref.so) and on libggml_b200 (H100); results are compared op by op and for whole
 LLaMA eval graphs (prompt + decode steps, KV cache carried across ggml_graph_compute calls).
 
 Bar: the reference library's BITS, op by op and at the logits of whole eval graphs -- every fp32 operation follows the reference's

@@ -7,7 +7,7 @@ sequence bit-exact"): the greedy token sequences are IDENTICAL and the logits of
 Tolerance zero: every fp32 operation of the path follows the reference's order (fastllama_b200/csrc/fl_exact.cuh) -- anything less
 exact ends up at the per-cent level after a few layers, because every activation vector is re-quantised to q8_0 before every matmul
 (DESIGN.md section 5; the round-1/early round-2 kernels, which only reordered the fp32 sums, measured 7.5e-2 of max|logit| at 32 layers
-and lost the token sequence at step 10).  A third case ingests a LONG prompt (>= 16 tokens: the tcgen05 GEMM, whose block terms are added
+and lost the token sequence at step 10).  A third case ingests a LONG prompt (>= 16 tokens: the wgmma GEMM, whose block terms are added
 in another order) and asserts the stated budget for that path, and bit equality again with FASTLLAMA_B200_INGEST=exact."""
 import os
 import sys
@@ -100,8 +100,8 @@ def test_13b_q4_1_four_layers_against_the_reference(tmp_path):
     finally:
         del os.environ["FASTLLAMA_B200_INGEST"]
     _check(ref_tokens, ref_logits, our_tokens, our_logits)
-    our_tokens, our_logits, _ = _ours(path, N_TOKENS, LONG_PROMPT, n_batch=128)     # default: tcgen05 GEMM for the prompt, reordering budget
+    our_tokens, our_logits, _ = _ours(path, N_TOKENS, LONG_PROMPT, n_batch=128)     # default: wgmma GEMM for the prompt, reordering budget
     par = bench.compare_parity(ref_tokens, ref_logits, our_tokens, our_logits)
-    print("parity (tcgen05 prompt ingest):", par)
+    print("parity (wgmma prompt ingest):", par)
     assert par["logits_maxabs_over_range"] <= LONG_TOL, par
     os.remove(path)

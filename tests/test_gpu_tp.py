@@ -1,4 +1,4 @@
-"""GPU (needs >= 2 B200 on the box; skipped otherwise): tensor-parallel decode (row-split matrices, activation vectors gathered over
+"""GPU (needs >= 2 GPUs on the box; skipped otherwise): tensor-parallel decode (row-split matrices, activation vectors gathered over
 NVLink as dataflow vectors inside the token kernel) against the single-GPU run: the same tokens and the same logit BITS.
 Launched like bench.py is: one process per GPU, rendezvous on 127.0.0.1."""
 import os

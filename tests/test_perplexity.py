@@ -1,6 +1,6 @@
 """Model.perplexity through the unchanged bridge (n_batch > 1 evals that return the logits of every token): the reference
 library vs our stack -- on the CPU stand-in of the device layer (host logic; its matmul is bit-identical to the reference's,
-so only the non-matmul ops differ) and on the B200 (tensor-core ingest kernel + generic executor)."""
+so only the non-matmul ops differ) and on the H100 (tensor-core ingest kernel + generic executor)."""
 import os
 import subprocess
 import sys

@@ -12,7 +12,7 @@ import random
 
 import pytest
 
-GRID = 148
+GRID = 132                  # one CTA per SM of an H100 SXM
 
 
 def magic(d):

@@ -115,7 +115,8 @@ wbytes = n_layer * (4 * n_embd * n_embd + 3 * n_ff * n_embd) // 32 * BB + n_voca
 print(f"{n_layer} layers + head: {ms.value / iters * 1e3:.1f} us per launch, {wbytes / (ms.value / iters * 1e-3) / 1e9:.0f} GB/s of weights")
 
 n_cta = C.c_int()
-prof = np.zeros((len(steps), 148, 4), dtype=np.uint64)
+n_sm = fl.device_props()["sm_count"]            # one CTA per SM
+prof = np.zeros((len(steps), n_sm, 4), dtype=np.uint64)
 fl.check(fl.lib.fl_token_plan_profile(plan, prof.ctypes.data, prof.size, C.byref(n_cta)))
 t = prof.astype(np.int64)
 t0 = t[0, :, 0].min()
@@ -137,7 +138,7 @@ for nm, rows in agg.items():
     r = np.array(rows).mean(axis=0)
     print(f"{nm:>5}: barrier {r[0]:5.2f} (max {r[1]:5.2f})  prologue {r[2]:5.2f} (max {r[3]:5.2f})  tiles {r[4]:5.2f} (max {r[5]:5.2f})  span {r[6]:6.2f}")
 # per-warp cycle breakdown of the tile loops (PROF kernel)
-p2 = np.zeros((len(steps), 148, 16, 8), dtype=np.uint32)
+p2 = np.zeros((len(steps), n_sm, 16, 8), dtype=np.uint32)
 fl.check(fl.lib.fl_token_plan_profile2(plan, p2.ctypes.data, p2.size))
 print("\nper consumer warp, mean over CTAs and warps (SM cycles): activation fetch | waiting for tiles | dots | reduce+epilogue+loop | rounds | total | tiles per CTA")
 agg2 = {}

@@ -1,4 +1,4 @@
-"""GPU probe: the tcgen05 prompt-ingest GEMM (fl_umma_kernel.cu; impl 5 / 6 / 7 = column tiles of 32 / 64 / 128) against the plain
+"""GPU probe: the wgmma prompt-ingest GEMM (fl_umma_kernel.cu; impl 5 / 6 / 7 = column tiles of 32 / 64 / 64) against the plain
 kernel (impl 1) and the exact oracle, then timings at the LLaMA-7B shapes.
 
   python tools/probe_umma.py [check|time|all]

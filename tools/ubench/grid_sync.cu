@@ -1,5 +1,5 @@
-// grid_sync.cu -- cost of a software grid barrier on B200, 148 CTAs x 544 threads (the token kernel's shape).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o grid_sync grid_sync.cu && ./grid_sync
+// grid_sync.cu -- cost of a software grid barrier, one CTA per SM x 544 threads (the token kernel's shape).
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o grid_sync grid_sync.cu && ./grid_sync
 #include <cstdio>
 #include <cuda_runtime.h>
 #define NT 512

@@ -1,6 +1,6 @@
 // Microbenchmark: how fast can one CTA per SM stream a contiguous HBM range into shared memory with
 // 1-D bulk copies (UBLKCP) through an mbarrier ring, with NO compute?  Sweeps tile size / stage count /
-// CTAs per SM.  Decides the ring geometry of the matvec kernels.   nvcc -arch=sm_100a -O3 tma_stream.cu
+// CTAs per SM.  Decides the ring geometry of the matvec kernels.   nvcc -arch=sm_90a -O3 tma_stream.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
