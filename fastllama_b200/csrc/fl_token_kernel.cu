@@ -17,7 +17,7 @@
 // rows), four lanes per row, lane jj carrying the reference's accumulators 2jj and 2jj+1 through ALL blocks of the row in order;
 // attention scores and the value mix follow ggml_vec_dot_f32's 32-lane order.  The logits of a token are therefore the bits the
 // reference's x86 build produces (the one known exception: rms_norm's double sum, see fl_ops_kernels.cu).
-// A task's rows are streamed in K-chunks of TK_CHB blocks: tile = (task, chunk) = 8 row pieces of <= 1280 (q4_0) / 1536 (q4_1)
+// A task's rows are streamed in K-chunks of TK_CHB blocks: tile = (task, chunk) = 8 row pieces of <= 640 (q4_0) / 768 (q4_1)
 // bytes, each copied by its own bulk copy to a row pitch of chunk + 16 bytes, which makes the 32 lanes' weight words fall into
 // 32 different banks.  The four consumer warps of a tile group take the tiles of their group's stream in turn.
 // Activations move between phases through L2: they are read with ld.global.cg (L1 is not coherent
@@ -39,7 +39,7 @@
 #define TK_TG 4                  // tile groups; ring slot s always belongs to group s % 4 (S is a multiple of 4)
 #define TK_WPG 4                 // consumer warps per tile group
 #define TK_GMAX 4                // units (row pairs) per task
-#define TK_CHB 64                // blocks per K-chunk of a task (one tile = 8 row pieces of one chunk)
+#define TK_CHB 32                // blocks per K-chunk of a task (one tile = 8 row pieces of one chunk; see DESIGN.md section 3 for 32 vs 64)
 #define TK_PW 4                  // producer warps: warp TK_CW + g streams the tiles of tile group g (its own slots, its own pace)
 #define TK_THREADS (TK_NT + 32 * TK_PW)
 #define TK_REGS_CONSUMER 104      // setmaxnreg: the producer warpgroup hands registers to the four consumer warpgroups.  The pool is the CTA's
@@ -81,7 +81,6 @@ struct tk_params {
     int S, Sg;                       // ring slots in total and per tile group (S = 4 * Sg)
     uint32_t grid_magic, grid_shift, s_magic, s_shift;  // n / d == umulhi(n, magic) >> shift (magic 0: d is a power of two, n >> shift); exact for n < 2^31; s_*: d = Sg
     uint32_t slot_bytes;
-    int l2_prefetch;
     int diag;                        // FASTLLAMA_B200_TK_DIAG (timing experiments only; results are garbage): 1 = no weight copies, 2 = no dot products, 4 = no grid barriers, 8 = no prologue
     uint32_t off_y, off_red, off_rowbuf, off_cnt, off_sc, off_stage0;
 };
@@ -800,6 +799,7 @@ __global__ void __launch_bounds__(TK_THREADS, 1) k_decode_token(const tk_params 
         } else if (pi > 0) {
             epoch++;
             if (!(prm.diag & 4)) tk_grid_sync(prm, epoch * gridDim.x, 0u);   // results of phase pi-1 are visible everywhere
+            else tk_bar_consumers(13);           // still a CTA barrier: sl_sh and phs[] are rewritten below while slower warps may read them
         }
         if (pr) pr[1] = tk_now();
         // Descriptor pi+1: the load is issued now, the store into phs[(pi+1)&1] (which nobody reads any more: everybody is
@@ -975,8 +975,6 @@ int flk_token_plan_create(const fl_token_step *steps, int n_steps, const uint16_
     tk_magic((uint32_t)p.Sg, p.s_magic, p.s_shift);
     p.slot_bytes = (uint32_t)slot;
     p.n_phases = n_steps;
-    // prefetching a whole phase competes with the demand loads of the phase still running, so it is opt-in
-    p.l2_prefetch = getenv("FASTLLAMA_B200_L2_PREFETCH") ? atoi(getenv("FASTLLAMA_B200_L2_PREFETCH")) : 0;
     p.exp_tab = exp_tab;
     p.diag = getenv("FASTLLAMA_B200_TK_DIAG") ? atoi(getenv("FASTLLAMA_B200_TK_DIAG")) : 0;
     pl->smem = off + (size_t)S * slot;
