@@ -12,6 +12,7 @@
 // block contributes fma(dx*dy, float(sum_i), acc) exactly as in the reference, only the order in
 // which the per-block terms are added in fp32 differs (lane-strided + shuffle tree here, 8 AVX
 // lanes there).
+#include <cuda_fp16.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -52,43 +53,85 @@ __global__ void k_quantize_q8_0(const float *__restrict__ x, size_t x_row_stride
 // =================================================================================================
 // q4_0 / q4_1 weight quantisation ("_reference" semantics: roundf = half away from zero)
 // =================================================================================================
+// One block per warp, element `lane` in v.  Writes the block and returns the lane's stored nibble
+// (the value ggml_quantize_q4_* counts in its histogram).
+__device__ __forceinline__ int fl_quantize_block_q4_0(float v, int lane, fl_block_q4_0 *yb) {
+    const float amax = fl_warp_max(fabsf(v));
+    const float d = __fdiv_rn(amax, 7.0f);
+    const float id = (d != 0.0f) ? __fdiv_rn(1.0f, d) : 0.0f;
+    const int q = (int)(int8_t)roundf(__fmul_rn(v, id)) + 8;
+    const int qn = __shfl_down_sync(0xffffffffu, q, 1);
+    if ((lane & 1) == 0) yb->qs[lane >> 1] = (uint8_t)((q & 0xFF) | (qn << 4));
+    if (lane == 0) yb->d = d;
+    return q & 0xF;
+}
+
+__device__ __forceinline__ int fl_quantize_block_q4_1(float v, int lane, fl_block_q4_1 *yb) {
+    float mn = v, mx = v;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    }
+    const float d = __fdiv_rn(__fsub_rn(mx, mn), 15.0f);
+    const float id = (d != 0.0f) ? __fdiv_rn(1.0f, d) : 0.0f;
+    const int q = (int)(uint8_t)roundf(__fmul_rn(__fsub_rn(v, mn), id));
+    const int qn = __shfl_down_sync(0xffffffffu, q, 1);
+    if ((lane & 1) == 0) yb->qs[lane >> 1] = (uint8_t)((q & 0xFF) | (qn << 4));
+    if (lane == 0) {
+        yb->d = d;
+        yb->m = mn;
+    }
+    return q & 0xF;
+}
+
 __global__ void k_quantize_q4_0(const float *__restrict__ x, fl_block_q4_0 *__restrict__ y, long nblocks) {
     const int lane = threadIdx.x & 31;
     const long wid = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const long nw = ((long)gridDim.x * blockDim.x) >> 5;
-    for (long b = wid; b < nblocks; b += nw) {
-        const float v = x[b * FL_QK + lane];
-        const float amax = fl_warp_max(fabsf(v));
-        const float d = __fdiv_rn(amax, 7.0f);
-        const float id = (d != 0.0f) ? __fdiv_rn(1.0f, d) : 0.0f;
-        const int q = (int)(int8_t)roundf(__fmul_rn(v, id)) + 8;
-        const int qn = __shfl_down_sync(0xffffffffu, q, 1);
-        if ((lane & 1) == 0) y[b].qs[lane >> 1] = (uint8_t)((q & 0xFF) | (qn << 4));
-        if (lane == 0) y[b].d = d;
-    }
+    for (long b = wid; b < nblocks; b += nw) fl_quantize_block_q4_0(x[b * FL_QK + lane], lane, y + b);
 }
 
 __global__ void k_quantize_q4_1(const float *__restrict__ x, fl_block_q4_1 *__restrict__ y, long nblocks) {
     const int lane = threadIdx.x & 31;
     const long wid = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const long nw = ((long)gridDim.x * blockDim.x) >> 5;
+    for (long b = wid; b < nblocks; b += nw) fl_quantize_block_q4_1(x[b * FL_QK + lane], lane, y + b);
+}
+
+// Model-file quantisation (the reference's fastllama::quantize, lib/llama.cpp:585-646): a tensor's
+// rows as the input file stores them, f32 or f16, to q4 blocks, plus the 16-bin histogram of the
+// stored nibbles that ggml_quantize_chunk reports.  f16 -> f32 is exact, so __half2float gives the
+// reference's ggml_fp16_to_fp32 inputs and the blocks carry the bits of k_quantize_q4_*.
+// Histogram: four ballots (one per bit of the nibble) give every lane the warp's count for bin
+// `lane` (lanes 0..15); the counts stay in a register across the warp's blocks, then go through
+// shared memory to one set of 16 64-bit global atomics per CTA.
+template <int TYPE, bool F16>
+__global__ void __launch_bounds__(256) k_quantize_q4_file(const void *__restrict__ x, void *__restrict__ y, long nblocks,
+                                                          unsigned long long *__restrict__ hist) {
+    __shared__ unsigned sh_hist[16];
+    const int lane = threadIdx.x & 31;
+    if (threadIdx.x < 16) sh_hist[threadIdx.x] = 0;
+    __syncthreads();
+    const long wid = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const long nw = ((long)gridDim.x * blockDim.x) >> 5;
+    unsigned cnt = 0;                                        // lanes 0..15: this warp's count of nibble value `lane`
     for (long b = wid; b < nblocks; b += nw) {
-        const float v = x[b * FL_QK + lane];
-        float mn = v, mx = v;
+        const float v = F16 ? __half2float(((const __half *)x)[b * FL_QK + lane]) : ((const float *)x)[b * FL_QK + lane];
+        const int q = (TYPE == FL_TYPE_Q4_0) ? fl_quantize_block_q4_0(v, lane, (fl_block_q4_0 *)y + b)
+                                             : fl_quantize_block_q4_1(v, lane, (fl_block_q4_1 *)y + b);
+        unsigned m = 0xffffffffu;
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        for (int j = 0; j < 4; j++) {
+            const unsigned plane = __ballot_sync(0xffffffffu, (q >> j) & 1);
+            m &= ((lane >> j) & 1) ? plane : ~plane;
         }
-        const float d = __fdiv_rn(__fsub_rn(mx, mn), 15.0f);
-        const float id = (d != 0.0f) ? __fdiv_rn(1.0f, d) : 0.0f;
-        const int q = (int)(uint8_t)roundf(__fmul_rn(__fsub_rn(v, mn), id));
-        const int qn = __shfl_down_sync(0xffffffffu, q, 1);
-        if ((lane & 1) == 0) y[b].qs[lane >> 1] = (uint8_t)((q & 0xFF) | (qn << 4));
-        if (lane == 0) {
-            y[b].d = d;
-            y[b].m = mn;
-        }
+        cnt += __popc(m);
+    }
+    if (hist) {
+        if (lane < 16 && cnt) atomicAdd(&sh_hist[lane], cnt);
+        __syncthreads();
+        if (threadIdx.x < 16 && sh_hist[threadIdx.x]) atomicAdd(hist + threadIdx.x, (unsigned long long)sh_hist[threadIdx.x]);
     }
 }
 
@@ -434,6 +477,26 @@ int flk_quantize_q4(cudaStream_t st, int type, const float *x, void *y, int k, i
         k_quantize_q4_0<<<grid_for_warps(nblocks, 256), 256, 0, st>>>(x, (fl_block_q4_0 *)y, nblocks);
     else
         k_quantize_q4_1<<<grid_for_warps(nblocks, 256), 256, 0, st>>>(x, (fl_block_q4_1 *)y, nblocks);
+    fl_count_launch();
+    FL_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+int flk_quantize_q4_file(cudaStream_t st, int type, int src_f16, const void *x, void *y, int k, int nrows,
+                         unsigned long long *hist) {
+    FL_REQUIRE(k > 0 && k % FL_QK == 0, "quantize_q4_file: k=%d is not a multiple of 32", k);
+    FL_REQUIRE(type == FL_TYPE_Q4_0 || type == FL_TYPE_Q4_1, "quantize_q4_file: unsupported type %d (q4_0 = 2, q4_1 = 3)", type);
+    FL_REQUIRE(src_f16 == 0 || src_f16 == 1, "quantize_q4_file: unsupported source type %d (0 f32, 1 f16)", src_f16);
+    if (nrows <= 0) return 0;
+    const long nblocks = (long)(k / FL_QK) * nrows;
+    const int grid = grid_for_warps(nblocks, 256);
+    if (type == FL_TYPE_Q4_0) {
+        if (src_f16) k_quantize_q4_file<FL_TYPE_Q4_0, true><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
+        else k_quantize_q4_file<FL_TYPE_Q4_0, false><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
+    } else {
+        if (src_f16) k_quantize_q4_file<FL_TYPE_Q4_1, true><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
+        else k_quantize_q4_file<FL_TYPE_Q4_1, false><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
+    }
     fl_count_launch();
     FL_CUDA_OK(cudaGetLastError());
     return 0;

@@ -8,6 +8,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <mutex>
 #include <vector>
 
 #include "fl_common.cuh"
@@ -35,6 +36,12 @@ struct State {
 };
 State g;
 thread_local char g_err[1024] = "";
+// fl_init / fl_shutdown may race when several host threads reach the library first at once.
+std::mutex g_init_mu;
+// The host-buffer entry points share the scratch slots: a larger request frees and reallocates a
+// slot, and every call stages its inputs there.  One caller at a time, from scratch_get to the
+// final stream synchronise; they all run on the one library stream anyway, so nothing is lost.
+std::mutex g_host_mu;
 }  // namespace
 
 void fl_set_error(const char *fmt, ...) {
@@ -121,6 +128,7 @@ static int ensure_rope(int n_dims, int n_pos) {
 // lifetime
 // ---------------------------------------------------------------------------------------------
 extern "C" int fl_init(int device) {
+    std::lock_guard<std::mutex> lk(g_init_mu);
     if (g.ready) return 0;
     int count = 0;
     cudaError_t e = cudaGetDeviceCount(&count);
@@ -149,6 +157,8 @@ extern "C" int fl_init(int device) {
 }
 
 extern "C" void fl_shutdown(void) {
+    std::lock_guard<std::mutex> lk(g_init_mu);
+    std::lock_guard<std::mutex> lk_host(g_host_mu);
     if (!g.ready) return;
     cudaStreamSynchronize(g.stream);
     for (auto &s : g.scratch) {
@@ -270,6 +280,12 @@ extern "C" int fl_dev_dequantize_rows(int type, const void *W, size_t wrs, int K
 extern "C" int fl_dev_quantize_q4(int type, const float *x, void *y, int k, int nrows) {
     FL_NEED_INIT();
     return flk_quantize_q4(g.stream, type, x, y, k, nrows);
+}
+
+extern "C" int fl_dev_quantize_q4_file(int type, int src_type, const void *x, void *y, int k, int nrows, unsigned long long *hist) {
+    FL_NEED_INIT();
+    FL_REQUIRE(x && y, "fl_dev_quantize_q4_file: null buffer");
+    return flk_quantize_q4_file(g.stream, type, src_type, x, y, k, nrows, hist);
 }
 
 extern "C" int fl_dev_quantize_q4_simd(int type, const float *x, void *y, int k, int nrows) {
@@ -691,6 +707,7 @@ extern "C" int fl_dev_time_mul_mat_q_rot(int type, const void *W, size_t wrs, in
                                          float *dst, size_t drs, int impl, int iters, size_t flush_l2_bytes,
                                          size_t copy_stride_bytes, int n_copies, float *ms_per_launch) {
     FL_NEED_INIT();
+    std::lock_guard<std::mutex> lk(g_host_mu);
     FL_REQUIRE(iters > 0 && ms_per_launch && n_copies >= 1, "fl_dev_time_mul_mat_q: bad arguments");
     const int mode = impl >> 8;
     impl &= 0xFF;
@@ -762,6 +779,7 @@ extern "C" int fl_dev_time_mul_mat_q_rot(int type, const void *W, size_t wrs, in
 // ---------------------------------------------------------------------------------------------
 extern "C" int fl_quantize_rows_q8_0(const float *x, void *y, int k, int nrows) {
     FL_NEED_INIT();
+    std::lock_guard<std::mutex> lk(g_host_mu);
     FL_REQUIRE(x && y && k > 0 && k % FL_QK == 0 && nrows >= 0, "fl_quantize_rows_q8_0: bad arguments (k=%d)", k);
     if (nrows == 0) return 0;
     const size_t xin = (size_t)k * nrows * sizeof(float), yout = (size_t)(k / FL_QK) * nrows * sizeof(fl_block_q8_0);
@@ -777,6 +795,7 @@ extern "C" int fl_quantize_row_q8_0(const float *x, void *y, int k) { return fl_
 
 extern "C" int fl_quantize_rows_q4(int type, const float *x, void *y, int k, int nrows) {
     FL_NEED_INIT();
+    std::lock_guard<std::mutex> lk(g_host_mu);
     FL_REQUIRE(x && y && k > 0 && k % FL_QK == 0 && nrows >= 0, "fl_quantize_rows_q4: bad arguments (k=%d)", k);
     FL_REQUIRE(type == FL_TYPE_Q4_0 || type == FL_TYPE_Q4_1, "fl_quantize_rows_q4: unsupported type %d", type);
     if (nrows == 0) return 0;
@@ -792,6 +811,7 @@ extern "C" int fl_quantize_rows_q4(int type, const float *x, void *y, int k, int
 
 extern "C" int fl_quantize_rows_q4_simd(int type, const float *x, void *y, int k, int nrows) {
     FL_NEED_INIT();
+    std::lock_guard<std::mutex> lk(g_host_mu);
     FL_REQUIRE(x && y && k > 0 && k % FL_QK == 0 && nrows >= 0, "fl_quantize_rows_q4_simd: bad arguments (k=%d)", k);
     FL_REQUIRE(type == FL_TYPE_Q4_0 || type == FL_TYPE_Q4_1, "fl_quantize_rows_q4_simd: unsupported type %d", type);
     if (nrows == 0) return 0;
@@ -807,6 +827,7 @@ extern "C" int fl_quantize_rows_q4_simd(int type, const float *x, void *y, int k
 
 extern "C" int fl_dequantize_rows_q4(int type, const void *x, float *y, int k, int nrows) {
     FL_NEED_INIT();
+    std::lock_guard<std::mutex> lk(g_host_mu);
     FL_REQUIRE(x && y && k > 0 && k % FL_QK == 0 && nrows >= 0, "fl_dequantize_rows_q4: bad arguments (k=%d)", k);
     FL_REQUIRE(type == FL_TYPE_Q4_0 || type == FL_TYPE_Q4_1, "fl_dequantize_rows_q4: unsupported type %d", type);
     if (nrows == 0) return 0;
@@ -823,6 +844,7 @@ extern "C" int fl_dequantize_rows_q4(int type, const void *x, float *y, int k, i
 
 extern "C" int fl_get_rows_q(int type, int K, int n_ids, const void *W, int n_rows_total, const int32_t *ids, float *dst) {
     FL_NEED_INIT();
+    std::lock_guard<std::mutex> lk(g_host_mu);
     FL_REQUIRE(W && ids && dst && K > 0 && K % FL_QK == 0, "fl_get_rows_q: bad arguments");
     FL_REQUIRE(type == FL_TYPE_Q4_0 || type == FL_TYPE_Q4_1, "fl_get_rows_q: unsupported type %d", type);
     for (int i = 0; i < n_ids; i++)
@@ -843,6 +865,7 @@ extern "C" int fl_get_rows_q(int type, int K, int n_ids, const void *W, int n_ro
 
 extern "C" int fl_vec_dot_q4_q8(int type, int n, float *s, const void *x, const void *y) {
     FL_NEED_INIT();
+    std::lock_guard<std::mutex> lk(g_host_mu);
     FL_REQUIRE(s && x && y && n > 0 && n % FL_QK == 0, "fl_vec_dot_q4_q8: bad arguments (n=%d)", n);
     FL_REQUIRE(type == FL_TYPE_Q4_0 || type == FL_TYPE_Q4_1, "fl_vec_dot_q4_q8: unsupported type %d", type);
     const size_t rb = (size_t)(n / FL_QK) * fl_block_bytes(type), qb = (size_t)(n / FL_QK) * sizeof(fl_block_q8_0);
@@ -858,6 +881,7 @@ extern "C" int fl_vec_dot_q4_q8(int type, int n, float *s, const void *x, const 
 
 extern "C" int fl_mul_mat_q_f32(int type, int M, int K, int N, const void *W, const float *X, float *dst) {
     FL_NEED_INIT();
+    std::lock_guard<std::mutex> lk(g_host_mu);
     FL_REQUIRE(W && X && dst && M >= 0 && N >= 0, "fl_mul_mat_q_f32: bad arguments");
     FL_REQUIRE(K > 0 && K % FL_QK == 0, "fl_mul_mat_q_f32: K=%d is not a multiple of 32", K);
     FL_REQUIRE(type == FL_TYPE_Q4_0 || type == FL_TYPE_Q4_1, "fl_mul_mat_q_f32: unsupported weight type %d", type);

@@ -609,11 +609,13 @@ std::vector<ggml_b200_kernel_stat> g_kstats;
 void *g_pev0 = nullptr, *g_pev1 = nullptr;
 
 void ensure_backend() {
-    static bool done = false;
-    if (done) return;
-    if (fl_init(-1) != 0) B200_FAIL("cannot initialise the B200 backend: %s", fl_last_error());
-    g_verbose = getenv("FASTLLAMA_B200_VERBOSE") != nullptr;
-    done = true;
+    // once per process, also when the first calls come from several threads at once (the reference's quantize tool calls
+    // ggml_quantize_chunk from a thread pool)
+    static std::once_flag once;
+    std::call_once(once, [] {
+        if (fl_init(-1) != 0) B200_FAIL("cannot initialise the B200 backend: %s", fl_last_error());
+        g_verbose = getenv("FASTLLAMA_B200_VERBOSE") != nullptr;
+    });
 }
 
 void drop_mirror(Mirror &m) {

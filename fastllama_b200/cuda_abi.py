@@ -130,6 +130,12 @@ SIGNATURES = {
     "fl_launch_count": (C.c_uint64, []),
 }
 
+# Bound on first use (FlCuda.fn) rather than at load, so that a stand-in library without them still loads for
+# everything else.  libfl_cuda.so exports them like every function of include/fl_cuda.h.
+LAZY_SIGNATURES = {
+    "fl_dev_quantize_q4_file": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+}
+
 
 class FlCuda:
     """Loaded libfl_cuda.so.  ``FlCuda(init=True)`` needs an H100."""
@@ -146,6 +152,14 @@ class FlCuda:
             self.check(self.lib.fl_init(device))
 
     # ---- helpers ---------------------------------------------------------------------------
+    def fn(self, name: str):
+        """An entry point of LAZY_SIGNATURES, typed; raises FlCudaError when the library lacks it."""
+        f = getattr(self.lib, name, None)
+        if f is None:
+            raise FlCudaError(f"{self.lib._name} does not export {name}")
+        f.restype, f.argtypes = LAZY_SIGNATURES[name]
+        return f
+
     def check(self, rc: int) -> None:
         if rc != 0:
             raise FlCudaError(f"libfl_cuda rc={rc}: {self.lib.fl_last_error().decode(errors='replace')}")

@@ -88,6 +88,57 @@ def write_ggjt(path: str, wtype: int, n_vocab: int, n_embd: int, n_mult: int, n_
         return f.tell()
 
 
+GGML_MAGIC, GGMF_MAGIC = 0x67676D6C, 0x67676D66
+F16 = 1
+FLOAT_DTYPE = {F32: np.float32, F16: np.float16}
+
+
+def write_model_file(path: str, fmt: str, hparams, vocab, tensors) -> int:
+    """Any single-file model the reference's reader accepts (include/file_loader.hpp:94-250).  fmt: "ggjt"
+    (version 1, tensor data 32-byte aligned), "ggmf" (version 1, no padding) or "ggml" (no version, vocab
+    without scores).  hparams: the 7 header integers; vocab: (bytes, score) pairs; tensors: (name, ne, type,
+    data bytes) with ne0 first."""
+    with open(path, "wb") as f:
+        if fmt == "ggml":
+            f.write(struct.pack("<I", GGML_MAGIC))
+        else:
+            f.write(struct.pack("<II", {"ggjt": GGJT_MAGIC, "ggmf": GGMF_MAGIC}[fmt], 1))
+        f.write(struct.pack("<7i", *hparams))
+        for tok, score in vocab:
+            f.write(struct.pack("<i", len(tok)) + tok + (b"" if fmt == "ggml" else struct.pack("<f", score)))
+        for name, ne, t, data in tensors:
+            nm = name.encode()
+            f.write(struct.pack("<iii", len(ne), len(nm), t))
+            f.write(struct.pack(f"<{len(ne)}i", *ne))
+            f.write(nm)
+            if fmt == "ggjt":
+                f.write(b"\0" * (-f.tell() & 31))
+            f.write(data)
+        return f.tell()
+
+
+def write_synthetic_float(path, ftype=F16, n_vocab=512, n_embd=256, n_mult=64, n_head=4, n_layer=2, seed=0, std=0.02,
+                          fmt="ggjt") -> int:
+    """An unquantised model as the reference's scripts/convert.py writes it: every 2-D tensor f16 (ftype 1) or
+    f32 (ftype 0), ~ N(0, std^2) (token embeddings N(0, 1)); 1-D norms f32 ones.  The input of the quantiser
+    (fastllama_b200/quantize.py).  Tensors are generated one at a time, so the host holds one at most."""
+    rng = np.random.default_rng(seed)
+    dt = FLOAT_DTYPE[ftype]
+
+    def tensors():
+        for name, ne in tensor_plan(n_vocab, n_embd, n_mult, n_head, n_layer):
+            if len(ne) == 1:
+                yield name, ne, F32, np.ones(ne[0], dtype=np.float32).tobytes()
+                continue
+            scale = 1.0 if name.startswith("tok_embeddings") else std
+            w = rng.standard_normal((ne[1], ne[0]), dtype=np.float32)
+            w *= np.float32(scale)
+            yield name, ne, ftype, w.astype(dt, copy=False).tobytes()
+
+    return write_model_file(path, fmt, (n_vocab, n_embd, n_mult, n_head, n_layer, n_embd // n_head, ftype),
+                            vocab_entries(n_vocab), tensors())
+
+
 def write_synthetic_numpy(path, wtype=Q4_0, n_vocab=512, n_embd=256, n_mult=64, n_head=4, n_layer=2, seed=0, std=0.02,
                           quantize=None) -> int:
     """CPU generator for toy models (tests).  `quantize(w_f32[M,K], wtype) -> uint8` must follow the

@@ -17,8 +17,12 @@
  *
  * Conventions: every function returning int returns 0 on success, negative on error
  * (fl_last_error() describes it).  There is no CPU fallback: without a CUDA device fl_init fails
- * and every other entry point fails with "not initialised".  Single caller thread (the reference
- * drives ggml from one thread, SURVEY.md 8b); all work is issued on one internal stream.
+ * and every other entry point fails with "not initialised".  All work is issued on one internal
+ * stream.  fl_init and the host-buffer entry points of group (1) may be called from several host
+ * threads at once (the reference's quantize tool calls ggml_quantize_chunk from a thread pool,
+ * lib/llama.cpp:613-645): one library mutex is held from the staging-buffer lookup to the final
+ * stream synchronise, so concurrent calls run one after another.  Everything else expects a
+ * single caller thread (the reference drives ggml from one thread, SURVEY.md 8b).
  */
 #ifndef FL_CUDA_H
 #define FL_CUDA_H
@@ -103,6 +107,14 @@ int fl_dev_mul_mat_q(int type, const void *W, size_t w_row_stride_bytes, int M, 
 int fl_dev_dequantize_rows(int type, const void *W, size_t w_row_stride_bytes, int K, const int32_t *ids_dev,
                            int n_ids, float *dst, size_t dst_row_stride_elems);
 int fl_dev_quantize_q4(int type, const float *x, void *y, int k, int nrows);
+
+/* Model-file quantisation (the tensor loop of fastllama::quantize, lib/llama.cpp:585-646): nrows rows
+ * of k elements as the input file stores them (src_type 0 = f32, 1 = f16; f16 converts exactly like
+ * ggml_fp16_to_fp32) -> q4_0 / q4_1 blocks with the bits of fl_quantize_rows_q4.  hist_dev (16
+ * counters, may be NULL) is incremented by the count of each stored nibble value, the histogram
+ * ggml_quantize_chunk reports.  Asynchronous on the library stream, like every fl_dev_* call. */
+int fl_dev_quantize_q4_file(int type, int src_type, const void *x_dev, void *y_dev, int k, int nrows,
+                            unsigned long long *hist_dev);
 
 /* ---- attach_lora / detach_lora on the device (reference lib/llama.cpp:697-944; SURVEY.md section 8 row f4) ----
  * fl_dev_quantize_q4_simd: device-resident fl_quantize_rows_q4_simd.
