@@ -18,6 +18,8 @@
 // fp16 value <= 1, i.e. a multiple of 2^-24); everything table-driven is exact.
 #include <cuda_fp16.h>
 
+#include <type_traits>
+
 #include "fl_common.cuh"
 #include "fl_kernels.h"
 
@@ -268,6 +270,41 @@ int flk_cpy_f32(cudaStream_t st, const fl_view &src, const fl_view &dst) {
     FL_REQUIRE(n == nelem(dst), "cpy: element counts differ");
     if (n <= 0) return 0;
     k_cpy_f32<<<ew_grid(n, 256), 256, 0, st>>>(src, dst, n);
+    fl_count_launch();
+    FL_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// tensor-parallel unshard: an all-gather of every rank's [N][n_local] slice leaves [world][N][n_local]; the eval needs
+// [N][world * n_local] (rank r's slice = elements [r * n_local, (r + 1) * n_local) of every row), optionally + residual, added
+// with one fp32 rounding per element as ggml_add does (reference lib/ggml.c:6259-6330).  V = 4: float4 loads and stores
+// (n_local % 4 == 0 and 16-byte aligned buffers), else one float at a time.
+// ------------------------------------------------------------------------------------------------
+template <int V>
+__global__ void k_tp_unshard(const float *__restrict__ g, int world, int N, int n_local, const float *res, float *dst) {
+    using T = typename std::conditional<V == 4, float4, float>::type;
+    const int nlv = n_local / V;
+    const int64_t row = (int64_t)world * nlv, n = (int64_t)N * row;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t col = i / row, c = i - col * row;
+        const int r = (int)(c / nlv), j = (int)(c - (int64_t)r * nlv);
+        T v = ((const T *)g)[((int64_t)r * N + col) * nlv + j];
+        if (res) {
+            const T b = ((const T *)res)[i];
+            if constexpr (V == 4) { v.x = __fadd_rn(v.x, b.x); v.y = __fadd_rn(v.y, b.y); v.z = __fadd_rn(v.z, b.z); v.w = __fadd_rn(v.w, b.w); }
+            else v = __fadd_rn(v, b);
+        }
+        ((T *)dst)[i] = v;
+    }
+}
+int flk_tp_unshard(cudaStream_t st, const float *gathered, int world, int N, int n_local, const float *residual, float *dst) {
+    FL_REQUIRE(gathered && dst && world >= 1 && N >= 0 && n_local >= 0, "tp_unshard: bad arguments");
+    const int64_t n = (int64_t)N * world * n_local;
+    if (n == 0) return 0;
+    const bool vec = n_local % 4 == 0 && (((uintptr_t)gathered | (uintptr_t)dst | (uintptr_t)residual) & 15) == 0;
+    if (vec) k_tp_unshard<4><<<ew_grid(n / 4, 256), 256, 0, st>>>(gathered, world, N, n_local, residual, dst);
+    else     k_tp_unshard<1><<<ew_grid(n, 256), 256, 0, st>>>(gathered, world, N, n_local, residual, dst);
     fl_count_launch();
     FL_CUDA_OK(cudaGetLastError());
     return 0;

@@ -348,6 +348,10 @@ extern "C" int fl_dev_mul_mat_f32(const fl_view *src0, const fl_view *src1, cons
     FL_NEED_INIT();
     return flk_mul_mat_f32(g.stream, *src0, *src1, *dst);
 }
+extern "C" int fl_dev_tp_unshard(const float *gathered, int world, int N, int n_local, const float *residual, float *dst) {
+    FL_NEED_INIT();
+    return flk_tp_unshard(g.stream, gathered, world, N, n_local, residual, dst);
+}
 
 // ---- fused decode step ------------------------------------------------------------------------
 extern "C" int fl_dev_mv_fused_supported(int type, int K, int mtot) { return flk_mv_fused_supported(type, K, mtot); }

@@ -28,6 +28,10 @@
 
 #include "fl_cuda.h"
 
+// Bound weakly, so that a device layer without it (one built before the tensor-parallel prompt plan, such as the CPU stand-in the
+// host-logic tests load) still loads: multi-token evals then keep the replicated executor (run_prompt_plan).  libfl_cuda.so exports it.
+extern "C" int fl_dev_tp_unshard(const float *gathered, int world, int N, int n_local, const float *residual, float *dst) __attribute__((weak));
+
 // ================================================================================================
 // small utilities
 // ================================================================================================
@@ -591,6 +595,7 @@ struct Mirror {
                              // ggml_set_scratch buffer (activations only, never uploaded)
     bool alive;
     bool device_dirty = false;   // a graph wrote into this persistent arena on the device (KV cache) since the last host sync
+    bool weights = false;        // the executor has read model weights through this mirror (ggml_b200_get_memory)
 };
 std::vector<Mirror> g_mirrors;
 int g_last_mirror = -1;
@@ -605,6 +610,8 @@ int64_t g_last_exit_us = 0;
 bool g_profile = false;
 int g_decode_mode = 0;          // see ggml_b200_decode_mode()
 bool g_tp_kv_sharded = false;   // tensor-parallel decode steps have written only this rank's heads into the KV cache
+uint64_t g_kv_gathers = 0;      // tp_gather_kv runs (ggml_b200_get_memory)
+int g_prompt_mode = 0;          // see ggml_b200_prompt_mode()
 std::vector<ggml_b200_kernel_stat> g_kstats;
 void *g_pev0 = nullptr, *g_pev1 = nullptr;
 
@@ -624,6 +631,7 @@ void drop_mirror(Mirror &m) {
         if (fl_is_initialized()) fl_dev_free(m.dev);
         m.dev = nullptr;
     }
+    m.weights = false;
 }
 
 int find_mirror(const void *p) {
@@ -763,6 +771,12 @@ static char *dev_ptr(const void *host, size_t nbytes, const ggml_context *comput
     }
     return m.dev + off;
 }
+// dev_ptr for a model weight (quantised matrix, norm weight, embedding table): counts its mirror in ggml_b200_get_memory
+static char *weight_ptr(const ggml_tensor *w, const ggml_context *compute_ctx) {
+    char *d = dev_ptr(w->data, nbytes_of(w), compute_ctx);
+    g_mirrors[find_mirror(w->data)].weights = true;
+    return d;
+}
 
 static void tp_gather_kv();
 // a device op is about to write `host`'s mirror: remember it if the arena is persistent (the KV cache)
@@ -869,15 +883,61 @@ struct Exec {
 };
 Exec g_exec;
 
-fl_view view_of(const ggml_tensor *t, const ggml_context *cctx) {
+inline bool in_ctx(const ggml_context *c, const void *p) {
+    return c && (const char *)p >= c->mem_buffer && (const char *)p < c->mem_buffer + c->mem_size;
+}
+// a tensor the graph reads but did not compute, outside its compute arena: a model weight (the KV cache is only ever read through views)
+inline bool is_weight_leaf(const ggml_tensor *t, const ggml_context *cctx) { return t && t->op == GGML_OP_NONE && t->data && !in_ctx(cctx, t->data); }
+
+// t's shape and strides over device memory `dev`
+fl_view view_at(const ggml_tensor *t, const void *dev) {
     fl_view v;
-    v.data = dev_ptr(t->data, nbytes_of(t), cctx);
+    v.data = (void *)dev;
     for (int i = 0; i < 4; i++) { v.ne[i] = t->ne[i]; v.nb[i] = (int64_t)t->nb[i]; }
     return v;
 }
+fl_view view_of(const ggml_tensor *t, const ggml_context *cctx) { return view_at(t, dev_ptr(t->data, nbytes_of(t), cctx)); }
 
 void need_f32(const ggml_tensor *t, const char *what) {
     if (t->type != GGML_TYPE_F32) B200_FAIL("%s: tensor type %s is not supported by the B200 backend (f32 only)", what, k_tname[t->type]);
+}
+
+// INIT phase of ggml_compute_forward_mul_mat_q_f32 (reference lib/ggml.c:8105-8119): N rows of K floats, x_row_stride_bytes apart ->
+// q8_0 rows in the executor's work buffer
+const void *quantize_cols_q8(const float *X, size_t x_row_stride_bytes, int K, int N) {
+    const size_t q8_bytes = (size_t)(K / 32) * 40 * (size_t)N;
+    if (g_exec.q8_cap < q8_bytes) {
+        if (g_exec.q8_work) FLC(fl_dev_free(g_exec.q8_work));
+        g_exec.q8_cap = std::max(q8_bytes, (size_t)1 << 20);
+        g_exec.q8_work = fl_dev_malloc(g_exec.q8_cap);
+        if (!g_exec.q8_work) B200_FAIL("q8_0 work buffer: %s", fl_last_error());
+    }
+    FLC(fl_dev_quantize_q8_0(X, x_row_stride_bytes, g_exec.q8_work, K, N));
+    return g_exec.q8_work;
+}
+
+// COMPUTE phase (reference lib/ggml.c:8125-8163): D[n * ldd + m] = W row m . Yq8 row n.  impl 0 is the executor's kernel choice, made
+// by the library from N alone: the reference-order kernel below 16 columns or under FASTLLAMA_B200_INGEST=exact, the wgmma GEMM
+// otherwise.  Both give every output the same fp32 order whatever M is, so a row slice of W yields the same bits as those rows of
+// the whole product (tests/test_gpu_tp_ingest.py) -- what the tensor-parallel prompt plan relies on.
+void mul_mat_q_cols(int type, const void *W, size_t w_row_stride, int M, int K, const void *Yq8, int N, float *D, size_t ldd) {
+    if (g_profile) FLC(fl_event_record(g_pev0));
+    FLC(fl_dev_mul_mat_q(type, W, w_row_stride, M, K, Yq8, N, D, ldd, 0));
+    if (g_profile) {
+        FLC(fl_event_record(g_pev1));
+        FLC(fl_event_sync(g_pev1));
+        float ms = 0.f;
+        FLC(fl_event_elapsed_ms(g_pev0, g_pev1, &ms));
+        ggml_b200_kernel_stat *e = nullptr;
+        for (auto &k : g_kstats) if (k.type == type && k.M == M && k.K == K && k.N == N) e = &k;
+        if (!e) {
+            g_kstats.push_back(ggml_b200_kernel_stat{type, M, K, N, 0, 0.0,
+                                                     (double)M * (K / 32) * (double)k_tsize[type] + (double)(K / 32) * 40.0 * N + 4.0 * M * N});
+            e = &g_kstats.back();
+        }
+        e->launches++;
+        e->total_ms += ms;
+    }
 }
 
 void exec_mul_mat(const ggml_tensor *node, const ggml_context *cctx) {
@@ -903,36 +963,11 @@ void exec_mul_mat(const ggml_tensor *node, const ggml_context *cctx) {
     B200_ASSERT(a->nb[0] == k_tsize[a->type] && b->nb[0] == sizeof(float) && node->nb[0] == sizeof(float));
     B200_ASSERT(a->ne[0] % 32 == 0 && a->ne[0] == b->ne[0]);
     const int M = (int)a->ne[1], K = (int)a->ne[0], N = (int)b->ne[1];
-    const size_t q8_bytes = (size_t)(K / 32) * 40 * (size_t)N;
-    if (g_exec.q8_cap < q8_bytes) {
-        if (g_exec.q8_work) FLC(fl_dev_free(g_exec.q8_work));
-        g_exec.q8_cap = std::max(q8_bytes, (size_t)1 << 20);
-        g_exec.q8_work = fl_dev_malloc(g_exec.q8_cap);
-        if (!g_exec.q8_work) B200_FAIL("q8_0 work buffer: %s", fl_last_error());
-    }
-    const char *W = dev_ptr(a->data, nbytes_of(a), cctx);
+    const char *W = weight_ptr(a, cctx);
     const float *X = (const float *)dev_ptr(b->data, nbytes_of(b), cctx);
     float *D = (float *)dev_ptr(node->data, nbytes_of(node), cctx);
-    // INIT phase: src1 rows -> q8_0 (reference lib/ggml.c:8105-8119)
-    FLC(fl_dev_quantize_q8_0(X, b->nb[1], g_exec.q8_work, K, N));
-    // COMPUTE phase (reference lib/ggml.c:8125-8163)
-    if (g_profile) FLC(fl_event_record(g_pev0));
-    FLC(fl_dev_mul_mat_q((int)a->type, W, a->nb[1], M, K, g_exec.q8_work, N, D, node->nb[1] / sizeof(float), 0));
-    if (g_profile) {
-        FLC(fl_event_record(g_pev1));
-        FLC(fl_event_sync(g_pev1));
-        float ms = 0.f;
-        FLC(fl_event_elapsed_ms(g_pev0, g_pev1, &ms));
-        ggml_b200_kernel_stat *e = nullptr;
-        for (auto &k : g_kstats) if (k.type == (int)a->type && k.M == M && k.K == K && k.N == N) e = &k;
-        if (!e) {
-            g_kstats.push_back(ggml_b200_kernel_stat{(int)a->type, M, K, N, 0, 0.0,
-                                                     (double)M * (K / 32) * (double)k_tsize[a->type] + (double)(K / 32) * 40.0 * N + 4.0 * M * N});
-            e = &g_kstats.back();
-        }
-        e->launches++;
-        e->total_ms += ms;
-    }
+    const void *Y = quantize_cols_q8(X, b->nb[1], K, N);
+    mul_mat_q_cols((int)a->type, W, a->nb[1], M, K, Y, N, D, node->nb[1] / sizeof(float));
 }
 
 void exec_node(ggml_tensor *node, const ggml_context *cctx) {
@@ -947,7 +982,7 @@ void exec_node(ggml_tensor *node, const ggml_context *cctx) {
             const ggml_tensor *a = node->src0, *ids = node->src1;
             if (a->type != GGML_TYPE_Q4_0 && a->type != GGML_TYPE_Q4_1)
                 B200_FAIL("get_rows: table type %s is not supported by the B200 backend (q4_0, q4_1)", k_tname[a->type]);
-            FLC(fl_dev_dequantize_rows((int)a->type, dev_ptr(a->data, nbytes_of(a), cctx), a->nb[1], (int)a->ne[0],
+            FLC(fl_dev_dequantize_rows((int)a->type, weight_ptr(a, cctx), a->nb[1], (int)a->ne[0],
                                        (const int32_t *)dev_ptr(ids->data, nbytes_of(ids), cctx), (int)ggml_nelements(ids),
                                        (float *)dev_ptr(node->data, nbytes_of(node), cctx), node->nb[1] / sizeof(float)));
             return;
@@ -965,7 +1000,7 @@ void exec_node(ggml_tensor *node, const ggml_context *cctx) {
                 need_f32(b, "add (quantised + f32) src1");
                 B200_ASSERT(node->type == a->type && same_shape(a, b) && same_shape(a, node) && a->ne[2] == 1 && a->ne[3] == 1);
                 B200_ASSERT(a->nb[0] == k_tsize[a->type] && b->nb[0] == sizeof(float) && node->nb[0] == k_tsize[a->type] && a->ne[0] % 32 == 0);
-                FLC(fl_dev_add_q_f32((int)a->type, dev_ptr(a->data, nbytes_of(a), cctx), a->nb[1], (int)a->ne[1], (int)a->ne[0],
+                FLC(fl_dev_add_q_f32((int)a->type, weight_ptr(a, cctx), a->nb[1], (int)a->ne[1], (int)a->ne[0],
                                      (const float *)dev_ptr(b->data, nbytes_of(b), cctx), b->nb[1] / sizeof(float), dev_ptr(node->data, nbytes_of(node), cctx), node->nb[1]));
                 // the host tensor follows the device (tensor-parallel shards are uploaded from the HOST tensor, and a mirror that is
                 // dropped later would otherwise come back with the unmerged bytes)
@@ -975,13 +1010,15 @@ void exec_node(ggml_tensor *node, const ggml_context *cctx) {
                 return;
             }
             need_f32(node->src0, k_opname[node->op]); need_f32(node->src1, k_opname[node->op]);
-            fl_view a = view_of(node->src0, cctx), b = view_of(node->src1, cctx), d = view_of(node, cctx);
+            // a one-token graph multiplies by the norm weight itself (no REPEAT node)
+            auto operand = [&](const ggml_tensor *t) { return is_weight_leaf(t, cctx) ? view_at(t, weight_ptr(t, cctx)) : view_of(t, cctx); };
+            fl_view a = operand(node->src0), b = operand(node->src1), d = view_of(node, cctx);
             if (node->op == GGML_OP_ADD) FLC(fl_dev_add(&a, &b, &d)); else FLC(fl_dev_mul(&a, &b, &d));
             return;
         }
         case GGML_OP_REPEAT: {
             need_f32(node->src0, "repeat");
-            fl_view s = view_of(node->src0, cctx), d = view_of(node, cctx);
+            fl_view s = is_weight_leaf(node->src0, cctx) ? view_at(node->src0, weight_ptr(node->src0, cctx)) : view_of(node->src0, cctx), d = view_of(node, cctx);
             FLC(fl_dev_repeat(&s, &d));
             return;
         }
@@ -1029,10 +1066,6 @@ void exec_node(ggml_tensor *node, const ggml_context *cctx) {
         default:
             B200_FAIL("op %s is outside the LLaMA eval set and has no B200 implementation (and there is no CPU fallback)", k_opname[node->op]);
     }
-}
-
-inline bool in_ctx(const ggml_context *c, const void *p) {
-    return c && (const char *)p >= c->mem_buffer && (const char *)p < c->mem_buffer + c->mem_size;
 }
 
 // ================================================================================================
@@ -1095,8 +1128,9 @@ struct DecodeState {
     size_t h_out_cap = 0;
     bool enabled = true, use_graph = true, use_token_kernel = true, inited = false;
     bool no_token_plan = false;       // the current plan's graph is not one the token kernel takes: node-by-node execution
-    bool tp_kv_sharded = false;   // tensor-parallel decode steps have written only this rank's heads into the KV cache ...
+    bool tp_kv_sharded = false;   // tensor-parallel decode steps / prompt-plan evals have written only this rank's heads into the KV cache ...
     int tp_first_pos = 0, tp_end_pos = 0;   // ... for positions [tp_first_pos, tp_end_pos)
+    struct { int n_embd = 0, n_ctx = 0; std::vector<float *> k, v; } tp_kv;   // that cache on the device: every layer's K [pos][n_embd], V [n_embd][n_ctx]
 };
 struct DecodeOutputs { const void *kv_host = nullptr; void *logits_host = nullptr; size_t logits_bytes = 0; void *emb_host = nullptr; size_t emb_bytes = 0; int32_t token = 0; };
 DecodeState g_dec;
@@ -1110,7 +1144,7 @@ struct Cur {
         return g->nodes[i++];
     }
 };
-#define PM(cond) do { if (!(cond)) { if (g_verbose) fprintf(stderr, "[ggml_b200] decode plan: no match (line %d): %s\n", __LINE__, #cond); return false; } } while (0)
+#define PM(cond) do { if (!(cond)) { if (g_verbose) fprintf(stderr, "[ggml_b200] eval plan: no match (line %d): %s\n", __LINE__, #cond); return false; } } while (0)
 
 inline bool is_qw(const ggml_tensor *w) {
     return w && w->op == GGML_OP_NONE && (w->type == GGML_TYPE_Q4_0 || w->type == GGML_TYPE_Q4_1) && w->ne[2] == 1 && w->ne[3] == 1 &&
@@ -1168,7 +1202,8 @@ void ensure_ws(DecodeWs &w, int n_embd, int n_ff, int n_vocab) {
 // [blk0, blk0 + nblk) of every row, gathered on the host into pinned staging so that the device never sees the other ranks' columns;
 // the packed row stride is a 16-byte multiple so every tile is still one bulk copy), or the whole tensor (norm weights, the
 // embedding table).  8 ranks of a 65B model upload 5 GB each instead of 40.6 GB.  The arena / mmap mirrors of the weights are not
-// touched by decode steps at all; a replicated multi-token eval (n_batch > 1) still mirrors what it reads.
+// touched by decode steps or by the tensor-parallel prompt plan (run_prompt_plan) at all: only an eval that falls back to the
+// replicated executor (FASTLLAMA_B200_TP_INGEST=replicated, or a graph the plans do not match) mirrors the weights it reads.
 struct ShardKey {
     const void *host; int kind, a, b;
     bool operator==(const ShardKey &o) const { return host == o.host && kind == o.kind && a == o.a && b == o.b; }
@@ -1225,100 +1260,174 @@ const void *tp_shard(const ggml_tensor *w, int kind, int a, int b, size_t *strid
     return dst;
 }
 
+// ---- Model::eval's graph, parsed once for the decode plan and the tensor-parallel prompt plan ----------------------------------------
+// The nodes of one layer (reference lib/llama.cpp:308-444) in the order ggml_build_forward_expand emits them.  With N > 1 columns every
+// norm weight passes through a REPEAT node; ggml_repeat returns its input when the shapes already agree (reference lib/ggml.c:4602-4604),
+// so a one-token graph has none.
+struct LayerNodes {
+    ggml_tensor *an, *arep, *ab;                              // attention norm: rms_norm, [repeat], mul
+    ggml_tensor *mk, *rsk, *rk, *vk, *ck;                     // K = rope(wk . x) -> its cache slots
+    ggml_tensor *mv, *rsv, *tv, *vv, *cv;                     // V = (wv . x)^T -> its cache slots
+    ggml_tensor *Vv, *Kv, *Kr, *Kp;                           // the cache as the attention reads it
+    ggml_tensor *mq, *rsq, *rq, *pq;                          // Q = rope(wq . x)
+    ggml_tensor *kq, *sc, *mask, *sm, *kqv, *pm, *att;        // attention
+    ggml_tensor *mo, *ff;                                     // wo, + residual
+    ggml_tensor *cn, *crep, *d, *m1, *s1, *m3, *h, *m2, *xo;  // feed-forward: norm, silu(w1 .) * (w3 .), w2, + residual
+    const ggml_tensor *attn_norm, *ffn_norm;                  // the norm weights
+};
+struct EvalGraph {
+    int N = 0, n_layer = 0, n_embd = 0, n_head = 0, hd = 0, n_past = -1, n_ctx = 0, n_ff = 0, n_vocab = 0;
+    float scale = 0.f;
+    ggml_tensor *emb = nullptr;                               // get_rows of the token embeddings
+    std::vector<LayerNodes> layers;
+    ggml_tensor *e = nullptr, *erep = nullptr, *f = nullptr;  // final norm; f = the embeddings
+    ggml_tensor *lg = nullptr;                                // LM head: the logits
+    const ggml_tensor *out_norm = nullptr;
+};
+// f32 [n0][n1] with dense rows
+inline bool is_rows(const ggml_tensor *t, int64_t n0, int64_t n1) {
+    return t && t->type == GGML_TYPE_F32 && t->ne[0] == n0 && t->ne[1] == n1 && t->ne[2] == 1 && t->ne[3] == 1 && t->nb[0] == 4 &&
+           (n1 == 1 || t->nb[1] == (size_t)n0 * 4);
+}
+
+// Checks, node for node, that g is Model::eval's graph for N tokens and collects its nodes.  The answer depends on the graph alone.
+bool parse_eval_graph(ggml_cgraph *g, EvalGraph &E) {
+    Cur c{g, 0, true};
+    ggml_tensor *n0 = c.next(GGML_OP_GET_ROWS);
+    PM(n0 && is_qw(n0->src0) && n0->src1 && n0->src1->type == GGML_TYPE_I32 && ggml_nelements(n0->src1) >= 1);
+    const int N = (int)ggml_nelements(n0->src1), rep = N > 1 ? 1 : 0;
+    const int per_layer = 37 + 2 * rep, fixed = 4 + rep;
+    PM(g->n_nodes >= fixed + per_layer && (g->n_nodes - fixed) % per_layer == 0);
+    const int n_embd = (int)n0->src0->ne[0];
+    PM(is_rows(n0, n_embd, N));
+    E.N = N; E.n_embd = n_embd; E.emb = n0;
+    E.n_layer = (g->n_nodes - fixed) / per_layer;
+    E.layers.resize(E.n_layer);
+    // rms_norm(x) times the norm weight (through a REPEAT node when N > 1)
+    auto norm = [&](const ggml_tensor *x, ggml_tensor *&nrm, ggml_tensor *&rp, ggml_tensor *&mul, const ggml_tensor *&gamma) {
+        nrm = c.next(GGML_OP_RMS_NORM);
+        rp = rep ? c.next(GGML_OP_REPEAT) : nullptr;
+        mul = c.next(GGML_OP_MUL);
+        if (!c.ok || nrm->src0 != x || mul->src1 != nrm || !is_rows(nrm, n_embd, N) || !is_rows(mul, n_embd, N)) return false;
+        if (rep && (mul->src0 != rp || rp->src1 != nrm || !is_rows(rp, n_embd, N))) return false;
+        gamma = rep ? rp->src0 : mul->src0;
+        return is_vec(gamma, n_embd) && gamma->op == GGML_OP_NONE;
+    };
+    const ggml_tensor *x = n0;
+    int n_past = -1, n_head = -1, n_ctx = -1, hd = 0;
+    for (int il = 0; il < E.n_layer; il++) {
+        LayerNodes &L = E.layers[il];
+        PM(norm(x, L.an, L.arep, L.ab, L.attn_norm));
+        const ggml_tensor *b = L.ab;
+        // K
+        L.mk = c.next(GGML_OP_MUL_MAT); L.rsk = c.next(GGML_OP_RESHAPE); L.rk = c.next(GGML_OP_ROPE); L.vk = c.next(GGML_OP_VIEW); L.ck = c.next(GGML_OP_CPY);
+        PM(c.ok && is_qw(L.mk->src0) && L.mk->src1 == b && L.rsk->src0 == L.mk && L.rk->src0 == L.rsk && L.ck->src0 == L.rk && L.ck->src1 == L.vk &&
+           is_rows(L.mk, n_embd, N));
+        if (il == 0) hd = (int)L.rsk->ne[0];
+        PM(hd > 0 && n_embd % hd == 0 && L.rsk->ne[0] == hd && L.rsk->ne[1] == n_embd / hd && L.rsk->ne[2] == N);
+        const int32_t *rp = (const int32_t *)L.rk->src1->data;
+        PM(rp[1] == hd && rp[2] == 0 && hd % 2 == 0);
+        if (il == 0) { n_past = rp[0]; n_head = n_embd / hd; }
+        PM(rp[0] == n_past && L.vk->type == GGML_TYPE_F32 && L.vk->src0 && L.vk->src0->op == GGML_OP_NONE && L.vk->ne[0] == (int64_t)N * n_embd &&
+           L.vk->nb[0] == 4);
+        // V
+        L.mv = c.next(GGML_OP_MUL_MAT); L.rsv = c.next(GGML_OP_RESHAPE); L.tv = c.next(GGML_OP_TRANSPOSE); L.vv = c.next(GGML_OP_VIEW); L.cv = c.next(GGML_OP_CPY);
+        PM(c.ok && is_qw(L.mv->src0) && L.mv->src1 == b && L.rsv->src0 == L.mv && L.tv->src0 == L.rsv && L.cv->src0 == L.tv && L.cv->src1 == L.vv &&
+           is_rows(L.mv, n_embd, N));
+        PM(L.vv->type == GGML_TYPE_F32 && L.vv->ne[0] == N && L.vv->ne[1] == n_embd && L.vv->nb[0] == 4 && L.vv->nb[1] % 4 == 0);
+        const int nctx_l = (int)(L.vv->nb[1] / 4);
+        if (il == 0) n_ctx = nctx_l;
+        PM(nctx_l == n_ctx && n_past + N <= n_ctx);
+        // cache views used by attention
+        L.Vv = c.next(GGML_OP_VIEW); L.Kv = c.next(GGML_OP_VIEW); L.Kr = c.next(GGML_OP_RESHAPE); L.Kp = c.next(GGML_OP_PERMUTE);
+        PM(c.ok && L.Kr->src0 == L.Kv && L.Kp->src0 == L.Kr && L.Vv->src0 == L.vv->src0 && L.Kv->src0 == L.vk->src0);
+        PM(L.Kv->ne[0] == (int64_t)(n_past + N) * n_embd && L.Vv->ne[0] == n_past + N && L.Vv->ne[1] == hd && L.Vv->ne[2] == n_head &&
+           L.Vv->nb[1] == (size_t)n_ctx * 4 && L.Vv->nb[2] == (size_t)n_ctx * 4 * hd);
+        // the slots this eval writes must be positions [n_past, n_past + N) of this layer's cache
+        PM((char *)L.vk->data == (char *)L.Kv->data + (size_t)n_past * n_embd * 4 && (char *)L.vv->data == (char *)L.Vv->data + (size_t)n_past * 4);
+        // Q
+        L.mq = c.next(GGML_OP_MUL_MAT); L.rsq = c.next(GGML_OP_RESHAPE); L.rq = c.next(GGML_OP_ROPE); L.pq = c.next(GGML_OP_PERMUTE);
+        PM(c.ok && is_qw(L.mq->src0) && L.mq->src1 == b && L.rsq->src0 == L.mq && L.rq->src0 == L.rsq && L.pq->src0 == L.rq && is_rows(L.mq, n_embd, N));
+        const int32_t *rpq = (const int32_t *)L.rq->src1->data;
+        PM(rpq[0] == n_past && rpq[1] == hd && rpq[2] == 0);
+        // attention
+        L.kq = c.next(GGML_OP_MUL_MAT); L.sc = c.next(GGML_OP_SCALE); L.mask = c.next(GGML_OP_DIAG_MASK_INF); L.sm = c.next(GGML_OP_SOFT_MAX);
+        L.kqv = c.next(GGML_OP_MUL_MAT); L.pm = c.next(GGML_OP_PERMUTE); L.att = c.next(GGML_OP_CPY);
+        PM(c.ok && L.kq->src0 == L.Kp && L.kq->src1 == L.pq && L.sc->src0 == L.kq && L.mask->src0 == L.sc && L.sm->src0 == L.mask && L.kqv->src0 == L.Vv &&
+           L.kqv->src1 == L.sm && L.pm->src0 == L.kqv && L.att->src0 == L.pm && is_rows(L.att, n_embd, N) && ggml_nelements(L.sc->src1) == 1 &&
+           L.sc->src1->op == GGML_OP_NONE);
+        PM(*(const int32_t *)L.mask->src1->data == n_past);
+        const float scale = *(const float *)L.sc->src1->data;
+        if (il == 0) E.scale = scale;
+        PM(scale == E.scale);
+        // output projection + residual
+        L.mo = c.next(GGML_OP_MUL_MAT); L.ff = c.next(GGML_OP_ADD);
+        PM(c.ok && is_qw(L.mo->src0) && L.mo->src1 == L.att && L.ff->src0 == L.mo && L.ff->src1 == x && is_rows(L.mo, n_embd, N) && is_rows(L.ff, n_embd, N));
+        // feed-forward
+        PM(norm(L.ff, L.cn, L.crep, L.d, L.ffn_norm));
+        L.m1 = c.next(GGML_OP_MUL_MAT); L.s1 = c.next(GGML_OP_SILU); L.m3 = c.next(GGML_OP_MUL_MAT); L.h = c.next(GGML_OP_MUL);
+        L.m2 = c.next(GGML_OP_MUL_MAT); L.xo = c.next(GGML_OP_ADD);
+        PM(c.ok && is_qw(L.m1->src0) && L.m1->src1 == L.d && L.s1->src0 == L.m1 && is_qw(L.m3->src0) && L.m3->src1 == L.d && L.h->src0 == L.s1 &&
+           L.h->src1 == L.m3 && is_qw(L.m2->src0) && L.m2->src1 == L.h && L.xo->src0 == L.m2 && L.xo->src1 == L.ff);
+        const ggml_tensor *wq = L.mq->src0, *wk = L.mk->src0, *wv = L.mv->src0, *wo = L.mo->src0, *w1 = L.m1->src0, *w3 = L.m3->src0, *w2 = L.m2->src0;
+        if (il == 0) E.n_ff = (int)w1->ne[1];
+        const int n_ff = E.n_ff;
+        PM(wq->type == wk->type && wq->type == wv->type && w1->type == w3->type);
+        PM(wq->ne[0] == n_embd && wk->ne[0] == n_embd && wv->ne[0] == n_embd && wq->ne[1] == n_embd && wk->ne[1] == n_embd && wv->ne[1] == n_embd);
+        PM(wo->ne[0] == n_embd && wo->ne[1] == n_embd && w1->ne[0] == n_embd && w1->ne[1] == n_ff && w3->ne[0] == n_embd && w3->ne[1] == n_ff &&
+           w2->ne[0] == n_ff && w2->ne[1] == n_embd);
+        PM(is_rows(L.m1, n_ff, N) && is_rows(L.s1, n_ff, N) && is_rows(L.m3, n_ff, N) && is_rows(L.h, n_ff, N) && is_rows(L.m2, n_embd, N) &&
+           is_rows(L.xo, n_embd, N));
+        x = L.xo;
+    }
+    PM(norm(x, E.e, E.erep, E.f, E.out_norm));
+    E.lg = c.next(GGML_OP_MUL_MAT);
+    PM(c.ok && c.i == g->n_nodes && is_qw(E.lg->src0) && E.lg->src1 == E.f && E.lg->src0->ne[0] == n_embd);
+    E.n_vocab = (int)E.lg->src0->ne[1];
+    PM(is_rows(E.lg, E.n_vocab, N));
+    E.n_head = n_head; E.hd = hd; E.n_past = n_past; E.n_ctx = n_ctx;
+    return n_past >= 0;
+}
+
 bool match_decode(const ggml_context *ctx, ggml_cgraph *g, DecodePlan &P, DecodeWs &W, DecodeOutputs &O) {
     const int world = fl_comm_world(), rank = fl_comm_rank();
     // weights: one GPU -> the arena / mmap mirror; tensor parallel -> only this rank's shard, uploaded from the host tensor (tp_shard)
-    auto wfull = [&](const ggml_tensor *t) -> const void * { return world == 1 ? (const void *)dp<const void>(t, ctx) : tp_shard(t, SH_FULL, 0, 0); };
+    auto wfull = [&](const ggml_tensor *t) -> const void * { return world == 1 ? (const void *)weight_ptr(t, ctx) : tp_shard(t, SH_FULL, 0, 0); };
     auto wrows = [&](const ggml_tensor *t, int row0, int n) -> const void * {
-        return world == 1 ? (const void *)((const char *)dp<const void>(t, ctx) + (size_t)row0 * t->nb[1]) : tp_shard(t, SH_ROWS, row0, n);
+        return world == 1 ? (const void *)(weight_ptr(t, ctx) + (size_t)row0 * t->nb[1]) : tp_shard(t, SH_ROWS, row0, n);
     };
-    PM(g->n_nodes >= 4 + 37 && (g->n_nodes - 4) % 37 == 0);
-    Cur c{g, 0, true};
-    ggml_tensor *n0 = c.next(GGML_OP_GET_ROWS);
-    PM(n0 && is_qw(n0->src0) && n0->src1 && n0->src1->type == GGML_TYPE_I32 && ggml_nelements(n0->src1) == 1);
-    const int n_embd = (int)n0->src0->ne[0];
-    PM(is_vec(n0, n_embd));
+    PM(g->n_nodes >= 4 + 37 && (g->n_nodes - 4) % 37 == 0);           // a one-token graph (no REPEAT nodes)
+    EvalGraph E;
+    if (!parse_eval_graph(g, E)) return false;
+    PM(E.N == 1);
+    const int n_embd = E.n_embd, n_head = E.n_head, n_ctx = E.n_ctx, n_past = E.n_past, hd = E.hd, n_ff = E.n_ff;
+    ggml_tensor *n0 = E.emb;
     P.n_embd = n_embd;
-    P.n_layer = (g->n_nodes - 4) / 37;
+    P.n_layer = E.n_layer;
     P.emb_type = (int)n0->src0->type; P.emb_K = n_embd; P.emb_stride = n0->src0->nb[1];
     P.emb_w = wfull(n0->src0);
     O.token = *(const int32_t *)n0->src1->data;
     P.layers.resize(P.n_layer);
-    ggml_tensor *x = n0;
-    int n_past = -1, n_head = -1, n_ctx = -1;
+    P.scale = E.scale;
     float *xin = nullptr, *xout = nullptr;     // residual stream ping-pong in the workspace
     for (int il = 0; il < P.n_layer; il++) {
         LayerPlan &L = P.layers[il];
-        ggml_tensor *a = c.next(GGML_OP_RMS_NORM), *b = c.next(GGML_OP_MUL);
-        PM(c.ok && a->src0 == x && b->src1 == a && is_vec(b->src0, n_embd) && b->src0->op == GGML_OP_NONE);
-        // K
-        ggml_tensor *mk = c.next(GGML_OP_MUL_MAT), *rsk = c.next(GGML_OP_RESHAPE), *rk = c.next(GGML_OP_ROPE), *vk = c.next(GGML_OP_VIEW),
-                    *ck = c.next(GGML_OP_CPY);
-        PM(c.ok && is_qw(mk->src0) && mk->src1 == b && rsk->src0 == mk && rk->src0 == rsk && ck->src0 == rk && ck->src1 == vk);
-        const int hd = (int)rsk->ne[0];
-        PM(hd > 0 && n_embd % hd == 0 && rsk->ne[1] == n_embd / hd && rsk->ne[2] == 1);
-        const int32_t *rp = (const int32_t *)rk->src1->data;
-        PM(rp[1] == hd && rp[2] == 0 && hd % 2 == 0);
-        if (il == 0) { n_past = rp[0]; n_head = n_embd / hd; }
-        PM(rp[0] == n_past && vk->type == GGML_TYPE_F32 && vk->src0 && vk->src0->op == GGML_OP_NONE);
-        // V
-        ggml_tensor *mvv = c.next(GGML_OP_MUL_MAT), *rsv = c.next(GGML_OP_RESHAPE), *tv = c.next(GGML_OP_TRANSPOSE), *vv = c.next(GGML_OP_VIEW),
-                    *cv = c.next(GGML_OP_CPY);
-        PM(c.ok && is_qw(mvv->src0) && mvv->src1 == b && rsv->src0 == mvv && tv->src0 == rsv && cv->src0 == tv && cv->src1 == vv);
-        PM(vv->type == GGML_TYPE_F32 && vv->ne[0] == 1 && vv->ne[1] == n_embd && vv->nb[1] % 4 == 0);
-        const int nctx_l = (int)(vv->nb[1] / 4);
-        if (il == 0) n_ctx = nctx_l;
-        PM(nctx_l == n_ctx && n_past < n_ctx);
-        // cache views used by attention
-        ggml_tensor *Vv = c.next(GGML_OP_VIEW), *Kv = c.next(GGML_OP_VIEW), *Kr = c.next(GGML_OP_RESHAPE), *Kp = c.next(GGML_OP_PERMUTE);
-        PM(c.ok && Kr->src0 == Kv && Kp->src0 == Kr && Vv->src0 == vv->src0 && Kv->src0 == vk->src0);
-        PM(Kv->ne[0] == (int64_t)(n_past + 1) * n_embd && Vv->ne[0] == n_past + 1 && Vv->ne[1] == hd && Vv->ne[2] == n_head &&
-           Vv->nb[1] == (size_t)n_ctx * 4 && Vv->nb[2] == (size_t)n_ctx * 4 * hd);
-        // the slots written this step must be position n_past of this layer's cache
-        PM((char *)vk->data == (char *)Kv->data + (size_t)n_past * n_embd * 4 && (char *)vv->data == (char *)Vv->data + (size_t)n_past * 4);
-        // Q
-        ggml_tensor *mq = c.next(GGML_OP_MUL_MAT), *rsq = c.next(GGML_OP_RESHAPE), *rq = c.next(GGML_OP_ROPE), *pq = c.next(GGML_OP_PERMUTE);
-        PM(c.ok && is_qw(mq->src0) && mq->src1 == b && rsq->src0 == mq && rq->src0 == rsq && pq->src0 == rq);
-        const int32_t *rpq = (const int32_t *)rq->src1->data;
-        PM(rpq[0] == n_past && rpq[1] == hd && rpq[2] == 0);
-        // attention
-        ggml_tensor *kq = c.next(GGML_OP_MUL_MAT), *sc = c.next(GGML_OP_SCALE), *mask = c.next(GGML_OP_DIAG_MASK_INF), *sm = c.next(GGML_OP_SOFT_MAX),
-                    *kqv = c.next(GGML_OP_MUL_MAT), *pm = c.next(GGML_OP_PERMUTE), *att = c.next(GGML_OP_CPY);
-        PM(c.ok && kq->src0 == Kp && kq->src1 == pq && sc->src0 == kq && mask->src0 == sc && sm->src0 == mask && kqv->src0 == Vv && kqv->src1 == sm &&
-           pm->src0 == kqv && att->src0 == pm && is_vec(att, n_embd) && ggml_nelements(sc->src1) == 1 && sc->src1->op == GGML_OP_NONE);
-        PM(*(const int32_t *)mask->src1->data == n_past);
-        const float scale = *(const float *)sc->src1->data;
-        if (il == 0) P.scale = scale;
-        PM(scale == P.scale);
-        // output projection + residual
-        ggml_tensor *mo = c.next(GGML_OP_MUL_MAT), *ff = c.next(GGML_OP_ADD);
-        PM(c.ok && is_qw(mo->src0) && mo->src1 == att && ff->src0 == mo && ff->src1 == x);
-        // feed-forward
-        ggml_tensor *cn = c.next(GGML_OP_RMS_NORM), *d = c.next(GGML_OP_MUL), *m1 = c.next(GGML_OP_MUL_MAT), *s1 = c.next(GGML_OP_SILU),
-                    *m3 = c.next(GGML_OP_MUL_MAT), *h = c.next(GGML_OP_MUL), *m2 = c.next(GGML_OP_MUL_MAT), *xo = c.next(GGML_OP_ADD);
-        PM(c.ok && cn->src0 == ff && d->src1 == cn && is_vec(d->src0, n_embd) && d->src0->op == GGML_OP_NONE && is_qw(m1->src0) && m1->src1 == d &&
-           s1->src0 == m1 && is_qw(m3->src0) && m3->src1 == d && h->src0 == s1 && h->src1 == m3 && is_qw(m2->src0) && m2->src1 == h &&
-           xo->src0 == m2 && xo->src1 == ff);
-        const ggml_tensor *wq = mq->src0, *wk = mk->src0, *wv = mvv->src0, *wo = mo->src0, *w1 = m1->src0, *w3 = m3->src0, *w2 = m2->src0;
-        const int n_ff = (int)w1->ne[1];
-        PM(wq->type == wk->type && wq->type == wv->type && w1->type == w3->type);
-        PM(wq->ne[0] == n_embd && wk->ne[0] == n_embd && wv->ne[0] == n_embd && wq->ne[1] == n_embd && wk->ne[1] == n_embd && wv->ne[1] == n_embd);
-        PM(wo->ne[0] == n_embd && wo->ne[1] == n_embd && w1->ne[0] == n_embd && w3->ne[0] == n_embd && w3->ne[1] == n_ff && w2->ne[0] == n_ff &&
-           w2->ne[1] == n_embd);
+        const LayerNodes &Ln = E.layers[il];
+        const ggml_tensor *wq = Ln.mq->src0, *wk = Ln.mk->src0, *wv = Ln.mv->src0, *wo = Ln.mo->src0, *w1 = Ln.m1->src0, *w3 = Ln.m3->src0, *w2 = Ln.m2->src0;
         PM(fl_dev_mv_fused_supported((int)wq->type, n_embd, 3 * n_embd) && fl_dev_mv_fused_supported((int)wo->type, n_embd, n_embd) &&
            fl_dev_mv_fused_supported((int)w1->type, n_embd, 2 * n_ff) && fl_dev_mv_fused_supported((int)w2->type, n_ff, n_embd));
 
-        if (world > 1) PM(n_head % world == 0 && n_ff % (32 * world) == 0 && (n_embd / world) % 32 == 0 && g->nodes[g->n_nodes - 1]->ne[0] % (2 * world) == 0);
+        if (world > 1) PM(n_head % world == 0 && n_ff % (32 * world) == 0 && (n_embd / world) % 32 == 0 && E.n_vocab % (2 * world) == 0);
         if (il == 0) {
-            ensure_ws(W, n_embd, n_ff, (int)g->nodes[g->n_nodes - 1]->ne[0]);
+            ensure_ws(W, n_embd, n_ff, E.n_vocab);
             P.emb_ids = W.d_tok; P.emb_dst = W.xa;
             xin = W.xa; xout = W.xb;
         }
         PM(W.n_ff == n_ff);
         L.q = W.q;
-        L.kcache = dp<const float>(Kv, ctx);
-        O.kv_host = Kv->data;
-        L.vcache = dp<const float>(Vv, ctx);
+        L.kcache = dp<const float>(Ln.Kv, ctx);
+        O.kv_host = Ln.Kv->data;
+        L.vcache = dp<const float>(Ln.Vv, ctx);
         L.att = W.att;
         // wq|wk|wv: rms_norm prologue, rope + cache-store epilogue
         mv_base(L.qkv, (int)wq->type, n_embd);
@@ -1327,7 +1436,7 @@ bool match_decode(const ggml_context *ctx, ggml_cgraph *g, DecodePlan &P, Decode
         L.qkv.seg_w[0] = wrows(wq, rank * nl_rows, nl_rows); L.qkv.seg_w[1] = wrows(wk, rank * nl_rows, nl_rows); L.qkv.seg_w[2] = wrows(wv, rank * nl_rows, nl_rows);
         L.qkv.seg_rows[0] = L.qkv.seg_rows[1] = L.qkv.seg_rows[2] = n_embd;
         L.qkv.seg_dst[0] = (float *)L.q;
-        L.qkv.pro = FL_PRO_RMSNORM; L.qkv.x = xin; L.qkv.gamma = (const float *)wfull(b->src0);
+        L.qkv.pro = FL_PRO_RMSNORM; L.qkv.x = xin; L.qkv.gamma = (const float *)wfull(Ln.attn_norm);
         L.qkv.epi = FL_EPI_QKV; L.qkv.n_ctx = n_ctx; L.qkv.n_embd = n_embd; L.qkv.head_dim = hd;
         L.qkv.kcache = (float *)L.kcache; L.qkv.vcache = (float *)L.vcache;
         // wo: plain prologue, residual epilogue
@@ -1339,7 +1448,7 @@ bool match_decode(const ggml_context *ctx, ggml_cgraph *g, DecodePlan &P, Decode
         const int fl_rows = n_ff / world;
         L.w13.nseg = 2; L.w13.seg_w[0] = wrows(w1, rank * fl_rows, fl_rows); L.w13.seg_w[1] = wrows(w3, rank * fl_rows, fl_rows);
         L.w13.seg_rows[0] = L.w13.seg_rows[1] = n_ff; L.w13.seg_dst[0] = W.m1; L.w13.seg_dst[1] = W.m3;
-        L.w13.pro = FL_PRO_RMSNORM; L.w13.x = W.ff; L.w13.gamma = (const float *)wfull(d->src0); L.w13.epi = FL_EPI_STORE;
+        L.w13.pro = FL_PRO_RMSNORM; L.w13.x = W.ff; L.w13.gamma = (const float *)wfull(Ln.ffn_norm); L.w13.epi = FL_EPI_STORE;
         // w2: silu*mul prologue, residual epilogue
         mv_base(L.w2, (int)w2->type, n_ff);
         L.w2.nseg = 1; L.w2.seg_w[0] = world == 1 ? wfull(w2) : nullptr; L.w2.seg_rows[0] = n_embd; L.w2.seg_dst[0] = xout;
@@ -1356,16 +1465,14 @@ bool match_decode(const ggml_context *ctx, ggml_cgraph *g, DecodePlan &P, Decode
             L.w13.seg_rows[0] = L.w13.seg_rows[1] = fl;
             L.w2.seg_w[0] = wrows(w2, rank * nl, nl); L.w2.seg_rows[0] = nl;
         }
-        x = xo;
         std::swap(xin, xout);
     }
-    ggml_tensor *e = c.next(GGML_OP_RMS_NORM), *f = c.next(GGML_OP_MUL), *lg = c.next(GGML_OP_MUL_MAT);
-    PM(c.ok && c.i == g->n_nodes && e->src0 == x && f->src1 == e && is_vec(f->src0, n_embd) && is_qw(lg->src0) && lg->src1 == f &&
-       lg->src0->ne[0] == n_embd && lg->src0->ne[1] % 2 == 0 && fl_dev_mv_fused_supported((int)lg->src0->type, n_embd, (int)lg->src0->ne[1]));
+    ggml_tensor *f = E.f, *lg = E.lg;
+    PM(lg->src0->ne[1] % 2 == 0 && fl_dev_mv_fused_supported((int)lg->src0->type, n_embd, (int)lg->src0->ne[1]));
     mv_base(P.head, (int)lg->src0->type, n_embd);
     P.head.nseg = 1; P.head.seg_w[0] = wrows(lg->src0, rank * (int)(lg->src0->ne[1] / world), (int)(lg->src0->ne[1] / world)); P.head.seg_rows[0] = (int)lg->src0->ne[1]; P.head.seg_dst[0] = W.logits;
     PM(W.n_vocab == (int)lg->src0->ne[1] && is_vec(lg, W.n_vocab) && is_vec(f, n_embd));
-    P.head.pro = FL_PRO_RMSNORM; P.head.x = xin; P.head.gamma = (const float *)wfull(f->src0); P.head.normed_out = W.emb;
+    P.head.pro = FL_PRO_RMSNORM; P.head.x = xin; P.head.gamma = (const float *)wfull(E.out_norm); P.head.normed_out = W.emb;
     O.logits_host = lg->data; O.logits_bytes = (size_t)W.n_vocab * 4; O.emb_host = f->data; O.emb_bytes = (size_t)n_embd * 4;
     P.world = world; P.heads_local = n_head / world;
     if (world > 1) {
@@ -1598,6 +1705,152 @@ bool run_decode_plan(const ggml_context *ctx, ggml_cgraph *g, DecodeOutputs &O, 
     g_stats.graph_replays++;
     return true;
 }
+
+// Tensor-parallel evals have written only this rank's heads of positions [first, end) into the KV cache
+void tp_kv_written(int first, int end) {
+    DecodeState &D = g_dec;
+    if (!D.tp_kv_sharded) { D.tp_first_pos = first; D.tp_end_pos = end; }
+    else { D.tp_first_pos = std::min(D.tp_first_pos, first); D.tp_end_pos = std::max(D.tp_end_pos, end); }
+    D.tp_kv_sharded = true; g_tp_kv_sharded = true;
+}
+
+// ================================================================================================
+// 3c. the tensor-parallel prompt plan
+//
+// A multi-token eval (a prompt, an n_batch chunk of one, a perplexity window) across `world` GPUs, lowered from the same parsed graph as
+// the decode plan and sharded the same way: wq/wk/wv by whole heads, w1/w3 by n_ff slices, wo, w2 and the output matrix by output rows.
+// Its weights are the decode plan's shards (tp_shard, same keys), so no rank ever holds a copy of the whole model.  Per layer, on every
+// rank:
+//   replicated  rms_norm * gamma of the whole [N][n_embd] residual stream and its q8_0 rows;
+//   local       the GEMMs on this rank's rows; rope, the KV-cache stores and the attention of this rank's heads (the executor's kernels
+//               on views restricted to those heads); silu * mul of this rank's n_ff slice;
+//   gathered    the attention output before wo, wo's output (+ residual), H before w2, w2's output (+ residual) and the logits: every
+//               rank's [N][n_local] slice is all-gathered, and fl_dev_tp_unshard writes the eval's [N][n] layout, adding the residual
+//               in the same pass.
+// Every element comes from the kernel the replicated executor runs for it, summed over the whole K on one GPU, so the ranks compute the
+// one-GPU bits.  The activations live where the executor keeps them, in the graph's own tensors; only the gather buffers are private.
+// The KV cache stays sharded by head: the attention of a later eval reads this rank's heads only, and tp_gather_kv runs before
+// save_state.
+// ================================================================================================
+struct PromptWs { float *send = nullptr, *recv = nullptr; size_t cap = 0; };   // this rank's [N][n_local] slice; the all-gather's [world][N][n_local]
+PromptWs g_pws;
+
+bool run_prompt_plan(const ggml_context *ctx, ggml_cgraph *g, void *ev0, void *ev1) {
+    const int world = fl_comm_world(), rank = fl_comm_rank();
+    // The decision depends on the graph, world, the switch and the device layer only, so every rank takes the same path (the gathers
+    // are collective).
+    if (world <= 1 || !fl_dev_tp_unshard || g->n_nodes < 5 + 39 || (g->n_nodes - 5) % 39 != 0) return false;
+    const char *sw = getenv("FASTLLAMA_B200_TP_INGEST");
+    if (sw && !strcmp(sw, "replicated")) return false;
+    EvalGraph E;
+    if (!parse_eval_graph(g, E) || E.N < 2) return false;
+    const int N = E.N, n_embd = E.n_embd, n_ff = E.n_ff, n_vocab = E.n_vocab, hd = E.hd, n_past = E.n_past;
+    if (E.n_head % world != 0 || n_ff % world != 0 || n_vocab % world != 0) return false;
+    const int hl = E.n_head / world, nl = n_embd / world, fl = n_ff / world, vl = n_vocab / world;
+    const size_t slice = ((size_t)N * std::max(nl, std::max(fl, vl)) + 63) & ~(size_t)63;      // floats; keeps recv 256-byte aligned
+    if (g_pws.cap < slice) {
+        if (g_pws.send) FLC(fl_dev_free(g_pws.send));
+        g_pws.send = (float *)fl_dev_malloc(slice * sizeof(float) * (size_t)(world + 1));
+        if (!g_pws.send) B200_FAIL("tensor-parallel prompt workspace: %s", fl_last_error());
+        g_pws.recv = g_pws.send + slice;
+        g_pws.cap = slice;
+    }
+    float *send = g_pws.send, *recv = g_pws.recv;
+
+    auto f32 = [&](const ggml_tensor *t) { return dp<float>(t, ctx); };
+    // v restricted to indices [first, first + n) of one axis
+    auto sub = [](fl_view v, int axis, int64_t first, int64_t n) { v.data = (char *)v.data + first * v.nb[axis]; v.ne[axis] = n; return v; };
+    auto dense3 = [](void *p, int64_t ne0, int64_t ne1, int64_t ne2, int64_t nb1, int64_t nb2) {
+        fl_view v;
+        v.data = p;
+        v.ne[0] = ne0; v.ne[1] = ne1; v.ne[2] = ne2; v.ne[3] = 1;
+        v.nb[0] = 4; v.nb[1] = nb1; v.nb[2] = nb2; v.nb[3] = nb2 * ne2;
+        return v;
+    };
+    auto q8_of = [&](const ggml_tensor *t) { return quantize_cols_q8(f32(t), t->nb[1], (int)t->ne[0], N); };
+    auto gemm = [&](const ggml_tensor *w, int row0, int rows, const void *q8, float *dst, size_t ldd) {
+        mul_mat_q_cols((int)w->type, tp_shard(w, SH_ROWS, row0, rows), w->nb[1], rows, (int)w->ne[0], q8, N, dst, ldd);
+    };
+    auto gather = [&](int n_local, const float *residual, float *dst) {
+        FLC(fl_comm_allgather_f32(send, recv, (size_t)N * n_local));
+        FLC(fl_dev_tp_unshard(recv, world, N, n_local, residual, dst));
+    };
+    auto norm = [&](const ggml_tensor *nrm, const ggml_tensor *rep, const ggml_tensor *mul, const ggml_tensor *gamma) {
+        fl_view s = view_of(nrm->src0, ctx), d = view_of(nrm, ctx);
+        FLC(fl_dev_rms_norm(&s, &d));
+        fl_view gv = view_at(gamma, tp_shard(gamma, SH_FULL, 0, 0)), r = view_of(rep, ctx);
+        FLC(fl_dev_repeat(&gv, &r));
+        fl_view a = view_of(mul->src0, ctx), b = view_of(mul->src1, ctx), o = view_of(mul, ctx);
+        FLC(fl_dev_mul(&a, &b, &o));
+    };
+
+    // the token ids are the one leaf a device op reads as data
+    const ggml_tensor *ids = E.emb->src1, *table = E.emb->src0;
+    const int32_t *ids_dev = (const int32_t *)dev_ptr(ids->data, nbytes_of(ids), ctx);
+    FLC(fl_h2d((void *)ids_dev, ids->data, nbytes_of(ids)));
+    FLC(fl_event_record(ev0));
+    FLC(fl_dev_dequantize_rows((int)table->type, tp_shard(table, SH_FULL, 0, 0), table->nb[1], n_embd, ids_dev, N, f32(E.emb), (size_t)n_embd));
+    for (const LayerNodes &L : E.layers) {
+        norm(L.an, L.arep, L.ab, L.attn_norm);
+        const void *q8 = q8_of(L.ab);
+        // K, V and Q of this rank's heads: rows [rank * nl, +nl) of wk / wv / wq, written to the same rows of the graph's [N][n_embd] results
+        gemm(L.mk->src0, rank * nl, nl, q8, f32(L.mk) + (size_t)rank * nl, n_embd);
+        fl_view k = sub(view_of(L.rk, ctx), 1, (int64_t)rank * hl, hl);
+        FLC(fl_dev_rope(&k, n_past, hd, 0));
+        mark_device_write(L.ck->data, ctx);
+        fl_view kslot = dense3((char *)f32(L.vk) + (size_t)rank * nl * 4, hd, hl, N, (int64_t)hd * 4, (int64_t)n_embd * 4);
+        FLC(fl_dev_cpy_f32(&k, &kslot));
+        gemm(L.mv->src0, rank * nl, nl, q8, f32(L.mv) + (size_t)rank * nl, n_embd);
+        fl_view v = sub(view_of(L.tv, ctx), 1, (int64_t)rank * nl, nl), vslot = sub(view_of(L.vv, ctx), 1, (int64_t)rank * nl, nl);
+        mark_device_write(L.cv->data, ctx);
+        FLC(fl_dev_cpy_f32(&v, &vslot));
+        gemm(L.mq->src0, rank * nl, nl, q8, f32(L.mq) + (size_t)rank * nl, n_embd);
+        fl_view q = sub(view_of(L.rq, ctx), 1, (int64_t)rank * hl, hl);
+        FLC(fl_dev_rope(&q, n_past, hd, 0));
+        // attention of this rank's heads (axis 2 of every operand)
+        auto heads = [&](const ggml_tensor *t) { return sub(view_of(t, ctx), 2, (int64_t)rank * hl, hl); };
+        fl_view K = heads(L.Kp), Q = heads(L.pq), S = heads(L.kq), sc = heads(L.sc), mk = heads(L.mask), sm = heads(L.sm), Vh = heads(L.Vv), O = heads(L.kqv);
+        FLC(fl_dev_mul_mat_f32(&K, &Q, &S));
+        FLC(fl_dev_scale(&sc, E.scale));
+        FLC(fl_dev_diag_mask_inf(&mk, n_past));
+        FLC(fl_dev_soft_max(&sm));
+        FLC(fl_dev_mul_mat_f32(&Vh, &sm, &O));
+        // this rank's heads of the merged [N][n_embd] attention output -> its [N][nl] slice; gather; wo on this rank's rows
+        fl_view pm = sub(view_of(L.pm, ctx), 1, (int64_t)rank * hl, hl), a = dense3(send, hd, hl, N, (int64_t)hd * 4, (int64_t)nl * 4);
+        FLC(fl_dev_cpy_f32(&pm, &a));
+        gather(nl, nullptr, f32(L.att));
+        gemm(L.mo->src0, rank * nl, nl, q8_of(L.att), send, nl);
+        gather(nl, f32(L.ff->src1), f32(L.ff));                                  // + the layer's input
+        // feed-forward: w1 / w3 on this rank's n_ff slice, silu * mul of it, gather H, w2 on this rank's rows
+        norm(L.cn, L.crep, L.d, L.ffn_norm);
+        const void *q8d = q8_of(L.d);
+        gemm(L.m1->src0, rank * fl, fl, q8d, f32(L.m1) + (size_t)rank * fl, n_ff);
+        gemm(L.m3->src0, rank * fl, fl, q8d, f32(L.m3) + (size_t)rank * fl, n_ff);
+        fl_view m1 = sub(view_of(L.m1, ctx), 0, (int64_t)rank * fl, fl), s1 = sub(view_of(L.s1, ctx), 0, (int64_t)rank * fl, fl);
+        FLC(fl_dev_silu(&m1, &s1));
+        fl_view m3 = sub(view_of(L.m3, ctx), 0, (int64_t)rank * fl, fl), hs = dense3(send, fl, N, 1, (int64_t)fl * 4, (int64_t)fl * 4 * N);
+        FLC(fl_dev_mul(&s1, &m3, &hs));
+        gather(fl, nullptr, f32(L.h));
+        gemm(L.m2->src0, rank * nl, nl, q8_of(L.h), send, nl);
+        gather(nl, f32(L.ff), f32(L.xo));                                        // + the attention block's output
+    }
+    norm(E.e, E.erep, E.f, E.out_norm);
+    gemm(E.lg->src0, rank * vl, vl, q8_of(E.f), send, vl);
+    gather(vl, nullptr, f32(E.lg));
+    FLC(fl_event_record(ev1));
+    // what the caller reads on the host (reference lib/llama.cpp:476-489): the logits of all N columns and the embeddings (the LM head's input)
+    FLC(fl_d2h(E.lg->data, f32(E.lg), nbytes_of(E.lg)));
+    FLC(fl_d2h(E.f->data, f32(E.f), nbytes_of(E.f)));
+    FLC(fl_sync());
+
+    DecodeState &D = g_dec;
+    D.tp_kv.n_embd = n_embd; D.tp_kv.n_ctx = E.n_ctx;
+    D.tp_kv.k.clear(); D.tp_kv.v.clear();
+    for (const LayerNodes &L : E.layers) { D.tp_kv.k.push_back(f32(L.Kv)); D.tp_kv.v.push_back(f32(L.Vv)); }
+    tp_kv_written(n_past, n_past + N);
+    if (g_verbose) fprintf(stderr, "[ggml_b200] tensor-parallel prompt plan: %d tokens from position %d, %d layers, rank %d of %d\n", N, n_past, E.n_layer, rank, world);
+    return true;
+}
 }  // namespace
 
 static void decode_state_release() {
@@ -1616,26 +1869,28 @@ static void decode_state_release() {
     D.no_token_plan = false;
     D.tp_kv_sharded = false;
     g_tp_kv_sharded = false;
+    D.tp_kv.k.clear(); D.tp_kv.v.clear();
     if (g_exec.q8_work) { fl_dev_free(g_exec.q8_work); g_exec.q8_work = nullptr; g_exec.q8_cap = 0; }
+    if (g_pws.send) { fl_dev_free(g_pws.send); g_pws = PromptWs(); }
 }
 
-// Tensor-parallel decode steps write only this rank's heads of the new positions into the KV cache (K [pos][n_embd]: nl
-// columns per row; V [n_embd][n_ctx]: nl rows).  Before anything reads the cache as a whole -- a replicated multi-token
-// eval, save_state -- the ranks exchange those slices: pack (strided copies) -> one all-gather -> unpack.  Collective.
+// Tensor-parallel decode steps and prompt-plan evals write only this rank's heads of the new positions into the KV cache (K [pos][n_embd]:
+// nl columns per row; V [n_embd][n_ctx]: nl rows).  Before anything reads the cache as a whole -- save_state, a replicated multi-token
+// eval -- the ranks exchange those slices: pack (strided copies) -> one all-gather -> unpack.  Collective.
 static void tp_gather_kv() {
     DecodeState &D = g_dec;
-    const DecodePlan &P = D.plan;
+    const auto &G = D.tp_kv;
     const int world = fl_comm_world(), rank = fl_comm_rank();
-    if (!D.tp_kv_sharded || world <= 1 || P.layers.empty()) { D.tp_kv_sharded = false; g_tp_kv_sharded = false; return; }
+    if (!D.tp_kv_sharded || world <= 1 || G.k.empty()) { D.tp_kv_sharded = false; g_tp_kv_sharded = false; return; }
     const int npos = D.tp_end_pos - D.tp_first_pos, first = D.tp_first_pos;
-    const int n_embd = P.n_embd, n_ctx = P.n_ctx, nl = n_embd / world, L = (int)P.layers.size();
+    const int n_embd = G.n_embd, n_ctx = G.n_ctx, nl = n_embd / world, L = (int)G.k.size();
     const size_t per_layer = (size_t)2 * npos * nl, count = per_layer * L;
     float *send = (float *)fl_dev_malloc(count * sizeof(float) * (size_t)(world + 1));
     if (!send) B200_FAIL("KV gather: %s", fl_last_error());
     float *recv = send + count;
     for (int l = 0; l < L; l++) {
-        const float *kmine = P.layers[l].kcache + (size_t)first * n_embd;                  // already offset to this rank's columns
-        const float *vmine = P.layers[l].vcache + first;                                   // already offset to this rank's rows
+        const float *kmine = G.k[l] + (size_t)first * n_embd + (size_t)rank * nl;          // this rank's columns of K [pos][n_embd]
+        const float *vmine = G.v[l] + (size_t)rank * nl * n_ctx + first;                   // this rank's rows of V [n_embd][n_ctx]
         FLC(fl_d2d_2d(send + l * per_layer, (size_t)nl * 4, kmine, (size_t)n_embd * 4, (size_t)nl * 4, (size_t)npos));
         FLC(fl_d2d_2d(send + l * per_layer + (size_t)npos * nl, (size_t)npos * 4, vmine, (size_t)n_ctx * 4, (size_t)npos * 4, (size_t)nl));
     }
@@ -1643,8 +1898,7 @@ static void tp_gather_kv() {
     for (int r = 0; r < world; r++) {
         if (r == rank) continue;
         for (int l = 0; l < L; l++) {
-            float *kbase = (float *)P.layers[l].kcache - (size_t)rank * nl;                // the layer's K [pos][n_embd]
-            float *vbase = (float *)P.layers[l].vcache - (size_t)rank * nl * n_ctx;        // the layer's V [n_embd][n_ctx]
+            float *kbase = G.k[l], *vbase = G.v[l];
             const float *src = recv + (size_t)r * count + l * per_layer;
             FLC(fl_d2d_2d(kbase + (size_t)first * n_embd + (size_t)r * nl, (size_t)n_embd * 4, src, (size_t)nl * 4, (size_t)nl * 4, (size_t)npos));
             FLC(fl_d2d_2d(vbase + (size_t)r * nl * n_ctx + first, (size_t)n_ctx * 4, src + (size_t)npos * nl, (size_t)npos * 4, (size_t)npos * 4, (size_t)nl));
@@ -1653,8 +1907,21 @@ static void tp_gather_kv() {
     FLC(fl_sync());
     FLC(fl_dev_free(send));
     if (g_verbose) fprintf(stderr, "[ggml_b200] gathered the KV cache of positions [%d, %d) from %d ranks\n", first, D.tp_end_pos, world);
+    g_kv_gathers++;
     D.tp_kv_sharded = false;
     g_tp_kv_sharded = false;
+}
+
+extern "C" int ggml_b200_prompt_mode(void) { return g_prompt_mode; }
+extern "C" void ggml_b200_get_memory(struct ggml_b200_memory *out) {
+    memset(out, 0, sizeof(*out));
+    for (const auto &m : g_mirrors) {
+        if (!m.alive || !m.dev) continue;
+        out->mirror_bytes += m.size;
+        if (m.weights) out->weight_mirror_bytes += m.size;
+    }
+    out->shard_bytes = g_shard_bytes;
+    out->kv_gathers = g_kv_gathers;
 }
 
 extern "C" void ggml_graph_compute(struct ggml_context *ctx, struct ggml_cgraph *g) {
@@ -1673,10 +1940,14 @@ extern "C" void ggml_graph_compute(struct ggml_context *ctx, struct ggml_cgraph 
         const int64_t t_issued = ggml_time_us();
         mark_device_write(dout.kv_host, ctx);          // the step appended one position to the KV cache on the device
         if (fl_comm_world() > 1) {
+            const DecodePlan &P = g_dec.plan;
+            const size_t own = (size_t)fl_comm_rank() * (size_t)(P.n_embd / P.world);     // the plan's cache pointers are offset to this rank's heads
+            auto &G = g_dec.tp_kv;
+            G.n_embd = P.n_embd; G.n_ctx = P.n_ctx;
+            G.k.clear(); G.v.clear();
+            for (const LayerPlan &L : P.layers) { G.k.push_back((float *)L.kcache - own); G.v.push_back((float *)L.vcache - own * P.n_ctx); }
             const int pos = g_dec.h_scalars[0];                   // n_past of this step = the position it wrote
-            if (!g_dec.tp_kv_sharded) { g_dec.tp_first_pos = pos; g_dec.tp_end_pos = pos + 1; }
-            else { g_dec.tp_first_pos = std::min(g_dec.tp_first_pos, pos); g_dec.tp_end_pos = std::max(g_dec.tp_end_pos, pos + 1); }
-            g_dec.tp_kv_sharded = true; g_tp_kv_sharded = true;
+            tp_kv_written(pos, pos + 1);
         }
         // fused decode step: the two results the caller reads (reference lib/llama.cpp:476-489) come
         // straight from the private workspace
@@ -1700,9 +1971,14 @@ extern "C" void ggml_graph_compute(struct ggml_context *ctx, struct ggml_cgraph 
         g_hostprof[3] += (double)(t_out - t_issued);
         if (g_last_exit_us) g_hostprof[4] += (double)(t_in - g_last_exit_us);
         g_last_exit_us = t_out;
+    } else if (run_prompt_plan(ctx, g, ev0, ev1)) {
+        g_last_exit_us = 0;
+        g_decode_mode = 0;
+        g_prompt_mode = 1;
     } else {
         g_last_exit_us = 0;
         g_decode_mode = 0;
+        if (g->n_nodes > 0 && g->nodes[0]->op == GGML_OP_GET_ROWS && g->nodes[0]->src1 && ggml_nelements(g->nodes[0]->src1) > 1) g_prompt_mode = 0;
         // Leafs.  Weights / KV cache live in persistent arenas (uploaded once by dev_ptr).  Constants the
         // host wrote into the compute arena while building the graph are uploaded per graph, but only
         // those a device op reads as DATA (token ids); rope / mask / scale parameters are read on the

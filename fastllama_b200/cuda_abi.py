@@ -134,6 +134,7 @@ SIGNATURES = {
 # everything else.  libfl_cuda.so exports them like every function of include/fl_cuda.h.
 LAZY_SIGNATURES = {
     "fl_dev_quantize_q4_file": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "fl_dev_tp_unshard": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
 }
 
 

@@ -161,6 +161,12 @@ int fl_dev_rope(const fl_view *t, int n_past, int n_dims, int mode);        /* i
 int fl_dev_cpy_f32(const fl_view *src, const fl_view *dst);
 int fl_dev_mul_mat_f32(const fl_view *src0, const fl_view *src1, const fl_view *dst);
 
+/* Tensor-parallel prompt ingest: fl_comm_allgather_f32 of every rank's [N][n_local] slice of a row-split result returns
+ * [world][N][n_local]; this writes the eval's layout [N][world * n_local] (rank r's slice at columns [r * n_local, +n_local) of
+ * every row).  residual (nullable, [N][world * n_local]) is added with one fp32 rounding per element -- the bits of ggml_add --
+ * so the gather after wo / w2 needs no separate add.  dst must not overlap `gathered`; it may be `residual`. */
+int fl_dev_tp_unshard(const float *gathered, int world, int N, int n_local, const float *residual, float *dst);
+
 /* ---- fused decode step (N = 1) ------------------------------------------------------------------
  * fl_dev_mv_fused: up to three weight matrices that share one input, one launch.  The prologue builds
  * the q8_0 activations from f32 inside the kernel (replacing rms_norm / mul / silu / quantize_row_q8_0

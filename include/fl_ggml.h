@@ -215,6 +215,17 @@ int ggml_b200_decode_mode(void);
 /* host-side time of the fused decode path in microseconds, summed over decode steps: [0] steps, [1] graph match, [2] match + scalars +
  * launch issue, [3] waiting for the device + result copies, [4] time spent in the caller between two decode steps */
 void ggml_b200_get_host_profile(double out[8], int reset);
+/* how the last multi-token eval ran: 0 = node-by-node executor (every rank replicated under tensor parallelism), 1 = tensor-parallel
+ * prompt plan (row-split matrices on this rank's weight shards, activations all-gathered; FASTLLAMA_B200_TP_INGEST=replicated forces 0) */
+int ggml_b200_prompt_mode(void);
+/* Device memory of this process:
+ *   weight_mirror_bytes: device mirrors of arenas / mmap ranges that the executor has read model weights from (0 on a
+ *                        tensor-parallel rank that has only run decode steps and prompt-plan evals: no rank copies the model);
+ *   shard_bytes:         tensor-parallel weight shards (this rank's rows of every matrix, norm weights, embedding table);
+ *   mirror_bytes:        all device mirrors (weights, KV cache, compute and scratch arenas);
+ *   kv_gathers:          all-gathers of a head-sharded KV cache run so far (save_state, or an eval that needs every head). */
+struct ggml_b200_memory { uint64_t weight_mirror_bytes, shard_bytes, mirror_bytes, kv_gathers; };
+void ggml_b200_get_memory(struct ggml_b200_memory *out);
 
 #ifdef __cplusplus
 }
