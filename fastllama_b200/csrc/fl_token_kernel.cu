@@ -661,20 +661,19 @@ __device__ __forceinline__ void tk_attention(const tk_phase &ph, const tk_params
         }
     }
 }
-// pull the cached positions of this head towards L2 while the grid is still finishing the previous phase
-__device__ __forceinline__ void tk_attention_prefetch(const tk_phase &ph, int head, int part_id, int tid) {
+// pull the cached positions of this head (all < n_past: the token's own row is stored in wq|wk|wv) towards L2.  The producer warps
+// (threads tid of nt) issue it when their walk reaches the attention, which is while the consumers still run wq|wk|wv: the transfer
+// then overlaps that phase's tile loop instead of the grid barrier in front of the attention (issued right before that barrier, it
+// made the barrier grow with n_past: 6.0 us at n_past 128, 9.7 us at 400 per layer on 7B).  Not inlined: inside the producer loop
+// (64 registers after setmaxnreg) it made ptxas spill.
+__device__ __noinline__ void tk_attention_prefetch(const tk_phase &ph, int head, int part_id, int tid, int nt) {
     const int hd = ph.head_dim, n_past = *ph.a.n_past;
-    const int kl = (hd * 4 + 127) / 128;                                  // 128-byte lines per cached K row of the head
-    for (int i = tid; i < n_past * kl; i += TK_NT) {
-        const float *p = ph.kcache + (size_t)(i / kl) * ph.k_row_stride + (size_t)head * hd + (i % kl) * 32;
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-    }
+    for (int j = tid; j < n_past; j += nt)                                // cached K rows of the head: hd floats each
+        for (int l = 0; l < hd; l += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(ph.kcache + (size_t)j * ph.k_row_stride + (size_t)head * hd + l));
     const int dpc = hd / ph.head_split;
-    const int vl = (n_past * 4 + 127) / 128;
-    for (int i = tid; i < dpc * vl; i += TK_NT) {
-        const float *p = ph.vcache + ((size_t)head * hd + part_id * dpc + i / vl) * ph.n_ctx + (i % vl) * 32;
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-    }
+    const float *v0 = ph.vcache + ((size_t)head * hd + (size_t)part_id * dpc) * ph.n_ctx;
+    for (int dl = 0; dl < dpc; dl++)                                      // cached V rows of this CTA's dimensions: n_past floats each
+        for (int l = 32 * tid; l < n_past; l += 32 * nt) asm volatile("prefetch.global.L2 [%0];" ::"l"(v0 + (size_t)dl * ph.n_ctx + l));
 }
 
 template <bool PROF>
@@ -720,7 +719,12 @@ __global__ void __launch_bounds__(TK_THREADS, 1) k_decode_token(const tk_params 
                 // The descriptor lives in global memory; everything the tile loop needs is pulled into registers once per phase
                 // (one L2 round trip, hidden because the producer runs ahead).
                 const tk_phase *gp = prm.phases + pi;
-                if (__ldg(&gp->kind) != TK_PH_MATVEC) continue;
+                if (__ldg(&gp->kind) != TK_PH_MATVEC) {                      // attention: its KV rows towards L2 (tk_attention_prefetch)
+                    const int hs = __ldg(&gp->head_split);
+                    if ((int)blockIdx.x < __ldg(&gp->n_head) * hs)
+                        tk_attention_prefetch(*gp, (int)blockIdx.x / hs, (int)blockIdx.x % hs, pg * 32 + lane, 32 * TK_PW);
+                    continue;
+                }
                 const int swiglu = __ldg(&gp->swiglu), C = __ldg(&gp->nchunks), nb = __ldg(&gp->nb), type = __ldg(&gp->a.type);
                 const int m0 = __ldg(&gp->units[0]), m1 = __ldg(&gp->units[1]), m2 = __ldg(&gp->units[2]);
                 const uint32_t row_bytes = __ldg(&gp->row_bytes), srow = __ldg(&gp->srow);
@@ -790,7 +794,6 @@ __global__ void __launch_bounds__(TK_THREADS, 1) k_decode_token(const tk_params 
         // attention: CTA b works on head b / head_split, output dimensions part b % head_split
         const bool attn_here = ph.kind == TK_PH_ATTN && (int)blockIdx.x < ph.n_head * ph.head_split;
         const int a_head = attn_here ? (int)blockIdx.x / ph.head_split : 0, a_part = attn_here ? (int)blockIdx.x % ph.head_split : 0;
-        if (attn_here) tk_attention_prefetch(ph, a_head, a_part, tid);
         const bool ll_in = ph.kind == TK_PH_MATVEC && ph.a.x_ll;      // input arrives element by element with epochs: no grid barrier at all
         const unsigned lle_in = ll_in ? ll_base + (unsigned)ph.a.x_seq + 1u : 0u;
         const unsigned lle_out = ph.kind == TK_PH_MATVEC ? (ph.a.out_ll ? ll_base + (unsigned)ph.a.out_seq + 1u : 0u) : (ph.out_ll ? ll_base + (unsigned)ph.out_seq + 1u : 0u);
