@@ -29,8 +29,12 @@ struct State {
     cudaStream_t stream = nullptr;
     uint16_t *tab_silu = nullptr;   // fp16 -> fp16 silu table (device)
     uint16_t *tab_exp = nullptr;    // fp16 -> fp16 exp table (device)
-    float2 *rope_cs = nullptr;      // [rope_pos][rope_dims/2]
-    int rope_dims = 0, rope_pos = 0;
+    // cos/sin tables, one per head dimension: [pos][dims/2] for positions [0, pos)
+    struct Rope { int dims = 0, pos = 0; float2 *cs = nullptr; };
+    std::vector<Rope> rope;
+    // Tables replaced by a larger one.  Programs and captured graphs of earlier decode plans still hold their addresses, so they stay
+    // allocated until fl_shutdown; capacity doubles on growth, so they add up to less than the live table of their head dimension.
+    std::vector<float2 *> rope_retired;
     Scratch scratch[4];
     uint64_t launches = 0;
 };
@@ -100,10 +104,16 @@ static int build_tables() {
 
 // rope cos/sin for absolute positions, computed with the reference's recurrence
 // (reference lib/ggml.c:8655-8668): theta_0 = (float)pos, theta_{i+1} = theta_i * powf(10000, -2/n_dims)
+static State::Rope *rope_of(int n_dims) {
+    for (auto &r : g.rope)
+        if (r.dims == n_dims) return &r;
+    return nullptr;
+}
 static int ensure_rope(int n_dims, int n_pos) {
-    if (g.rope_cs && g.rope_dims == n_dims && g.rope_pos >= n_pos) return 0;
+    State::Rope *r = rope_of(n_dims);
+    if (r && r->pos >= n_pos) return 0;
     int cap = n_pos < 512 ? 512 : n_pos;
-    if (g.rope_dims == n_dims && cap < 2 * g.rope_pos) cap = 2 * g.rope_pos;
+    if (r && cap < 2 * r->pos) cap = 2 * r->pos;
     const int half = n_dims / 2;
     std::vector<float2> cs((size_t)cap * half);
     const float theta_scale = powf(10000.0, -2.0f / n_dims);
@@ -114,13 +124,18 @@ static int ensure_rope(int n_dims, int n_pos) {
             theta *= theta_scale;
         }
     }
-    FL_CUDA_OK(cudaStreamSynchronize(g.stream));
-    if (g.rope_cs) FL_CUDA_OK(cudaFree(g.rope_cs));
-    g.rope_cs = nullptr;
-    FL_CUDA_OK(cudaMalloc((void **)&g.rope_cs, cs.size() * sizeof(float2)));
-    FL_CUDA_OK(cudaMemcpy(g.rope_cs, cs.data(), cs.size() * sizeof(float2), cudaMemcpyHostToDevice));
-    g.rope_dims = n_dims;
-    g.rope_pos = cap;
+    float2 *d = nullptr;
+    FL_CUDA_OK(cudaMalloc((void **)&d, cs.size() * sizeof(float2)));
+    FL_CUDA_OK(cudaMemcpy(d, cs.data(), cs.size() * sizeof(float2), cudaMemcpyHostToDevice));
+    if (!r) {
+        g.rope.push_back(State::Rope());
+        r = &g.rope.back();
+    } else {
+        g.rope_retired.push_back(r->cs);
+    }
+    r->dims = n_dims;
+    r->pos = cap;
+    r->cs = d;
     return 0;
 }
 
@@ -167,7 +182,8 @@ extern "C" void fl_shutdown(void) {
     }
     if (g.tab_silu) cudaFree(g.tab_silu);
     if (g.tab_exp) cudaFree(g.tab_exp);
-    if (g.rope_cs) cudaFree(g.rope_cs);
+    for (auto &r : g.rope) cudaFree(r.cs);
+    for (float2 *p : g.rope_retired) cudaFree(p);
     flk_exact_release();
     cudaStreamDestroy(g.stream);
     g = State();
@@ -338,7 +354,8 @@ extern "C" int fl_dev_rope(const fl_view *t, int n_past, int n_dims, int mode) {
     FL_NEED_INIT();
     const int need = (int)(((mode & 1) ? 0 : n_past) + t->ne[2]);
     if (ensure_rope(n_dims, need) != 0) return -1;
-    return flk_rope(g.stream, *t, n_past, n_dims, mode, g.rope_cs, g.rope_pos);
+    const State::Rope *r = rope_of(n_dims);
+    return flk_rope(g.stream, *t, n_past, n_dims, mode, r->cs, r->pos);
 }
 extern "C" int fl_dev_cpy_f32(const fl_view *src, const fl_view *dst) {
     FL_NEED_INIT();
@@ -365,9 +382,9 @@ extern "C" int fl_dev_mv_fused(const fl_mv_args *args) {
     FL_REQUIRE(a.n_dst_peer == 0 && !a.x_ll && !a.out_ll && !a.res_ll, "fl_dev_mv_fused: dataflow (LL) vectors and peer outputs exist only inside the token kernel");
     a.silu_tab = g.tab_silu;
     if (a.epi == FL_EPI_QKV) {
-        FL_REQUIRE(g.rope_cs && g.rope_dims == a.head_dim && g.rope_pos >= a.n_ctx,
-                   "fl_dev_mv_fused: call fl_dev_rope_table(head_dim, n_ctx) first (table must not move under a captured graph)");
-        a.rope_cs = g.rope_cs;
+        const State::Rope *r = rope_of(a.head_dim);
+        FL_REQUIRE(r && r->pos >= a.n_ctx, "fl_dev_mv_fused: call fl_dev_rope_table(head_dim, n_ctx) first");
+        a.rope_cs = r->cs;
     }
     return flk_mv_fused(g.stream, &a);
 }
@@ -380,11 +397,14 @@ extern "C" int fl_token_plan_create(const fl_token_step *steps, int n_steps, voi
 extern "C" int fl_token_plan_create_ll(const fl_token_step *steps, int n_steps, unsigned *epoch_counter, void **plan_out) {
     FL_NEED_INIT();
     FL_REQUIRE(steps && n_steps > 0 && plan_out, "fl_token_plan_create: bad arguments");
+    const State::Rope *rope = nullptr;
     for (int i = 0; i < n_steps; i++)
-        if (steps[i].kind == 0 && steps[i].mv.epi == FL_EPI_QKV)
-            FL_REQUIRE(g.rope_cs && g.rope_dims == steps[i].mv.head_dim && g.rope_pos >= steps[i].mv.n_ctx,
-                       "fl_token_plan_create: call fl_dev_rope_table(head_dim, n_ctx) first");
-    return flk_token_plan_create(steps, n_steps, g.tab_silu, g.tab_exp, g.rope_cs, epoch_counter, plan_out);
+        if (steps[i].kind == 0 && steps[i].mv.epi == FL_EPI_QKV) {
+            const State::Rope *r = rope_of(steps[i].mv.head_dim);
+            FL_REQUIRE(r && r->pos >= steps[i].mv.n_ctx && (!rope || rope == r), "fl_token_plan_create: call fl_dev_rope_table(head_dim, n_ctx) first");
+            rope = r;
+        }
+    return flk_token_plan_create(steps, n_steps, g.tab_silu, g.tab_exp, rope ? rope->cs : nullptr, epoch_counter, plan_out);
 }
 extern "C" int fl_token_plan_launch(void *plan) {
     FL_NEED_INIT();

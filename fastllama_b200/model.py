@@ -157,11 +157,12 @@ class Model:
         if getattr(self, "ctx", None):
             self.lib.llama_free_context(self.ctx)
             self.ctx = None
-            # The bridge has no hook for device memory, so the mirror of the reference API does it: every device allocation of the
-            # backend (weights / KV mirrors, decode plan, workspace) is released, and a later model can never see this one's weights.
-            # (A library without the symbol -- the reference build the tests use as CPU oracle -- has nothing to release.)
+            # The bridge has no hook for device memory, so the mirror of the reference API does it: the device allocations of this
+            # context (weights / KV mirrors, decode state, its share of the workspaces) are released, and a later model can never see
+            # its weights.  Other live contexts keep theirs.  (A library without the symbol -- the reference build the tests use as
+            # CPU oracle -- has nothing to release.)
             try:
-                release = self.lib.ggml_b200_release_all
+                release = self.lib.ggml_b200_release_unused
             except AttributeError:
                 release = None
             if release is not None:

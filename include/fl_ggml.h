@@ -198,8 +198,22 @@ quantize_fns_t ggml_internal_get_quantize_fn(size_t i);
 void ggml_b200_invalidate(const void *ptr, size_t size);
 /* Copy a device-resident range back to its host arena (KV cache before save_state). */
 void ggml_b200_sync_to_host(const void *ptr, size_t size);
-/* Drop every device mirror (model unload). */
+/* Free every device resource of the backend: all contexts' mirrors, decode states, shards and workspaces (all models unloaded). */
 void ggml_b200_release_all(void);
+/* Free the device resources of everything whose host memory is gone: mirrors of freed arenas and of unmapped or remapped file ranges,
+ * decode states of freed contexts, tensor-parallel shards of freed weights, and the shared workspaces once no context is left.  Live
+ * contexts keep everything, their device-written KV caches included.  fastllama_b200.Model.close() calls it after llama_free_context;
+ * after the last context it leaves the device as ggml_b200_release_all does. */
+void ggml_b200_release_unused(void);
+/* Contexts of this process:
+ *   live_states:       decode states (one per context that has run an eval on the fused plans; released with the context);
+ *   plan_builds:       token-kernel programs built so far (a plan is built once per context and shape, not per switch);
+ *   graph_captures:    decode steps captured into a CUDA graph so far;
+ *   external_copies:   device copies of mmap'ed weight ranges, keyed by (file, offset): mappings of one file share them;
+ *   external_mappings: live mapped ranges using those copies (> external_copies when contexts share a file);
+ *   external_bytes:    bytes of those copies. */
+struct ggml_b200_contexts { uint64_t live_states, plan_builds, graph_captures, external_copies, external_mappings, external_bytes; };
+void ggml_b200_get_contexts(struct ggml_b200_contexts *out);
 /* Counters for bench.py: evals run, device microseconds of the last eval (CUDA events), kernels launched */
 struct ggml_b200_stats { uint64_t n_evals; double last_eval_device_us; double total_device_us; uint64_t launches; uint64_t graph_replays; };
 void ggml_b200_get_stats(struct ggml_b200_stats *out);
