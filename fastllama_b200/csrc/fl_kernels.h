@@ -58,6 +58,9 @@ int flk_mul_mat_q_umma(cudaStream_t st, int type, const void *W, size_t w_row_st
 int flk_quantize_q4_simd(cudaStream_t st, int type, const float *x, void *y, int k, int nrows);
 int flk_add_q_f32(cudaStream_t st, int type, const void *W, size_t w_row_stride, int M, int K, const float *X, size_t x_row_stride_elems, void *dst,
                   size_t dst_row_stride);
+int flk_add_q_f16(cudaStream_t st, int type, const void *W, size_t w_row_stride, int M, int K, const uint16_t *X, size_t x_row_stride_elems, void *dst,
+                  size_t dst_row_stride);
+int flk_scale_f16(cudaStream_t st, uint16_t *x, long n, float v);
 int flk_mul_mat_f32_ref(cudaStream_t st, const float *A, size_t lda, int Ma, const float *B, size_t ldb, int Mb, int K, float *out, size_t ldo);
 
 // fl_exact_kernels.cu: results with the reference's fp32 bits (fl_exact.cuh): q4 x q8_0 matmul for any M, K, N, and the f32 mul_mat

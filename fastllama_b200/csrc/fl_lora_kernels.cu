@@ -6,7 +6,13 @@
 // dequantize_row_q, ggml_vec_acc_f32, quantize_row_q -- the SIMD quantiser (AVX2 branches :739-803 and :965-1038), whose
 // arithmetic differs from the _reference quantisers that define file contents:
 //   q4_0: id = 7 / amax (not 1 / (amax / 7)), round-half-EVEN; q4_1: round-half-EVEN.
-// Everything here is bit-exact against the reference's x86 build (tests/golden/lora_ops.npz, produced by the reference library).
+// A cached adapter stored as f16 (convert-lora-to-ggml.py --dtype fp16) takes ggml_compute_forward_add_q_f16 (lib/ggml.c:12372-12483)
+// instead: the same row loop with X widened from f16 -- and detach first negates it in place with ggml_compute_forward_scale_f16
+// (:12485-12524).
+// Everything here is bit-exact against the reference's x86 build (tests/golden/lora_ops.npz and lora_f16_ops.npz, produced by the
+// reference library).
+#include <cuda_fp16.h>
+
 #include "fl_common.cuh"
 #include "fl_exact.cuh"
 #include "fl_kernels.h"
@@ -57,10 +63,15 @@ __global__ void k_quantize_q4_simd(const float *__restrict__ x, uint8_t *__restr
     }
 }
 
-// ggml_compute_forward_add_q_f32: dst row = quantize_row_q(dequantize_row_q(src0 row) + src1 row); dst may alias src0 (add_inplace)
-template <int TYPE>
-__global__ void k_add_q_f32(const uint8_t *W, size_t w_row_stride, int M, int K, const float *__restrict__ X, size_t x_row_stride, uint8_t *D,
-                            size_t d_row_stride) {
+// X's element as fp32: f32 as is; f16 widened exactly (GGML_FP16_TO_FP32, the F16C build's _cvtsh_ss)
+__device__ __forceinline__ float lq_widen(float x) { return x; }
+__device__ __forceinline__ float lq_widen(uint16_t x) { return __half2float(__ushort_as_half(x)); }
+
+// ggml_compute_forward_add_q_f32 (XT = float) and ggml_compute_forward_add_q_f16 (XT = uint16_t, f16 bits): dst row =
+// quantize_row_q(dequantize_row_q(src0 row) + fp32(src1 row)); dst may alias src0 (add_inplace)
+template <int TYPE, typename XT>
+__global__ void k_add_q(const uint8_t *W, size_t w_row_stride, int M, int K, const XT *__restrict__ X, size_t x_row_stride, uint8_t *D,
+                        size_t d_row_stride) {
     constexpr int BB = (TYPE == FL_TYPE_Q4_0) ? 20 : 24;
     constexpr int QOFF = (TYPE == FL_TYPE_Q4_0) ? 4 : 8;
     const int nb = K / FL_QK;
@@ -77,12 +88,19 @@ __global__ void k_add_q_f32(const uint8_t *W, size_t w_row_stride, int M, int K,
         float v;
         if (TYPE == FL_TYPE_Q4_0) v = __fmul_rn((float)(code - 8), d);                       // dequantize_row_q4_0, lib/ggml.c:1449-1481
         else v = __fmaf_rn((float)code, d, *(const float *)(src + 4));                       // dequantize_row_q4_1 (fused in the GNU-mode build), :1567-1596
-        v = __fadd_rn(v, X[(size_t)r * x_row_stride + (size_t)ib * FL_QK + lane]);           // ggml_vec_acc_f32, :2286
+        v = __fadd_rn(v, lq_widen(X[(size_t)r * x_row_stride + (size_t)ib * FL_QK + lane])); // ggml_vec_acc_f32 :2286 / the f16 loop :12476-12478
         __syncwarp();                                                                        // every lane has read the block before it is overwritten in place
         uint8_t *dst = D + (size_t)r * d_row_stride + (size_t)ib * BB;
         const int q = lq_quantize_simd<TYPE>(v, lane, dst);
         lq_store_codes<TYPE>(q, lane, dst);
     }
+}
+
+// ggml_compute_forward_scale_f16 (ggml_scale is a view, so this is in place): x = fp16_rn(fp32(x) * v), the F16C build's
+// _cvtsh_ss / _cvtss_sh(., 0)
+__global__ void k_scale_f16(uint16_t *x, long n, float v) {
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
+        x[i] = __half_as_ushort(__float2half_rn(__fmul_rn(lq_widen(x[i]), v)));
 }
 
 // ggml_mul_mat on two f32 matrices in the reference's summation order (ggml_vec_dot_f32, lib/ggml.c:2295-2325, AVX2 + FMA build):
@@ -148,16 +166,33 @@ int flk_quantize_q4_simd(cudaStream_t st, int type, const float *x, void *y, int
     return 0;
 }
 
-int flk_add_q_f32(cudaStream_t st, int type, const void *W, size_t w_row_stride, int M, int K, const float *X, size_t x_row_stride_elems, void *dst,
-                  size_t dst_row_stride) {
-    FL_REQUIRE(K > 0 && K % FL_QK == 0, "add_q_f32: K=%d is not a multiple of 32", K);
-    FL_REQUIRE(type == FL_TYPE_Q4_0 || type == FL_TYPE_Q4_1, "add_q_f32: unsupported type %d", type);
+template <typename XT>
+static int add_q(cudaStream_t st, int type, const void *W, size_t w_row_stride, int M, int K, const XT *X, size_t x_row_stride_elems, void *dst,
+                 size_t dst_row_stride) {
+    FL_REQUIRE(K > 0 && K % FL_QK == 0, "add_q: K=%d is not a multiple of 32", K);
+    FL_REQUIRE(type == FL_TYPE_Q4_0 || type == FL_TYPE_Q4_1, "add_q: unsupported type %d", type);
     if (M <= 0) return 0;
     const long nblocks = (long)(K / FL_QK) * M;
     if (type == FL_TYPE_Q4_0)
-        k_add_q_f32<FL_TYPE_Q4_0><<<lq_grid(nblocks, 256), 256, 0, st>>>((const uint8_t *)W, w_row_stride, M, K, X, x_row_stride_elems, (uint8_t *)dst, dst_row_stride);
+        k_add_q<FL_TYPE_Q4_0, XT><<<lq_grid(nblocks, 256), 256, 0, st>>>((const uint8_t *)W, w_row_stride, M, K, X, x_row_stride_elems, (uint8_t *)dst, dst_row_stride);
     else
-        k_add_q_f32<FL_TYPE_Q4_1><<<lq_grid(nblocks, 256), 256, 0, st>>>((const uint8_t *)W, w_row_stride, M, K, X, x_row_stride_elems, (uint8_t *)dst, dst_row_stride);
+        k_add_q<FL_TYPE_Q4_1, XT><<<lq_grid(nblocks, 256), 256, 0, st>>>((const uint8_t *)W, w_row_stride, M, K, X, x_row_stride_elems, (uint8_t *)dst, dst_row_stride);
+    fl_count_launch();
+    FL_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+int flk_add_q_f32(cudaStream_t st, int type, const void *W, size_t w_row_stride, int M, int K, const float *X, size_t x_row_stride_elems, void *dst,
+                  size_t dst_row_stride) {
+    return add_q(st, type, W, w_row_stride, M, K, X, x_row_stride_elems, dst, dst_row_stride);
+}
+int flk_add_q_f16(cudaStream_t st, int type, const void *W, size_t w_row_stride, int M, int K, const uint16_t *X, size_t x_row_stride_elems, void *dst,
+                  size_t dst_row_stride) {
+    return add_q(st, type, W, w_row_stride, M, K, X, x_row_stride_elems, dst, dst_row_stride);
+}
+
+int flk_scale_f16(cudaStream_t st, uint16_t *x, long n, float v) {
+    if (n <= 0) return 0;
+    k_scale_f16<<<lq_grid((n + 31) / 32, 256), 256, 0, st>>>(x, n, v);
     fl_count_launch();
     FL_CUDA_OK(cudaGetLastError());
     return 0;

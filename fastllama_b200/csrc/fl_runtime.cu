@@ -313,6 +313,21 @@ extern "C" int fl_dev_add_q_f32(int type, const void *W, size_t w_row_stride_byt
     FL_NEED_INIT();
     return flk_add_q_f32(g.stream, type, W, w_row_stride_bytes, M, K, X, x_row_stride_elems, dst, dst_row_stride_bytes);
 }
+extern "C" int fl_dev_add_q_f16(int type, const void *W, size_t w_row_stride_bytes, int M, int K, const uint16_t *X, size_t x_row_stride_elems, void *dst,
+                                size_t dst_row_stride_bytes) {
+    FL_NEED_INIT();
+    return flk_add_q_f16(g.stream, type, W, w_row_stride_bytes, M, K, X, x_row_stride_elems, dst, dst_row_stride_bytes);
+}
+extern "C" int fl_dev_scale_f16(const fl_view *t, float v) {
+    FL_NEED_INIT();
+    int64_t n = 1, nb = 2;
+    for (int i = 0; i < 4; i++) {
+        FL_REQUIRE(t->nb[i] == nb, "fl_dev_scale_f16: the tensor is not contiguous f16 (nb[%d] = %lld)", i, (long long)t->nb[i]);
+        nb *= t->ne[i];
+        n *= t->ne[i];
+    }
+    return flk_scale_f16(g.stream, (uint16_t *)t->data, (long)n, v);
+}
 extern "C" int fl_dev_mul_mat_f32_ref(const float *A, size_t lda, int Ma, const float *B, size_t ldb, int Mb, int K, float *out, size_t ldo) {
     FL_NEED_INIT();
     return flk_mul_mat_f32_ref(g.stream, A, lda, Ma, B, ldb, Mb, K, out, ldo);

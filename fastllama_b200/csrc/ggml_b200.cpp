@@ -35,6 +35,11 @@
 // Bound weakly, so that a device layer without it (one built before the tensor-parallel prompt plan, such as the CPU stand-in the
 // host-logic tests load) still loads: multi-token evals then keep the replicated executor (run_prompt_plan).  libfl_cuda.so exports it.
 extern "C" int fl_dev_tp_unshard(const float *gathered, int world, int N, int n_local, const float *residual, float *dst) __attribute__((weak));
+// The f16 ops of a cached f16 LoRA adapter, bound weakly for the same reason: a device layer without them still loads and runs everything
+// else, and an f16 adapter on it fails with an error naming the missing entry point.  libfl_cuda.so exports both.
+extern "C" int fl_dev_add_q_f16(int type, const void *W, size_t w_row_stride_bytes, int M, int K, const uint16_t *X, size_t x_row_stride_elems,
+                                void *dst, size_t dst_row_stride_bytes) __attribute__((weak));
+extern "C" int fl_dev_scale_f16(const fl_view *t, float v) __attribute__((weak));
 
 // ================================================================================================
 // small utilities
@@ -690,6 +695,10 @@ Mirror &mirror_alloc(Mirror &m) {
 }  // namespace
 
 static void packed_shards_clear();
+// Shards were dropped (a LoRA merge rewrote weights, or their host range went away): the ranks come back to the next decode step after
+// work of their own -- a merge has no collective, and the shards are cut again -- so that step lines them up even when the plan's
+// device pointers happen to be unchanged and nothing is rebuilt.
+static bool g_tp_realign = false;
 namespace {
 // one line of /proc/self/maps: [lo, hi), file offset, device and inode (inode 0: anonymous memory)
 struct MapEntry { uintptr_t lo, hi; unsigned long off, dev, ino; };
@@ -1064,13 +1073,30 @@ void exec_node(ggml_tensor *node, const ggml_context *cctx) {
         }
         case GGML_OP_ADD: case GGML_OP_MUL: {
             if (node->op == GGML_OP_ADD && (node->src0->type == GGML_TYPE_Q4_0 || node->src0->type == GGML_TYPE_Q4_1)) {
-                // W (+)= f32 matrix: the LoRA merge, ggml_compute_forward_add_q_f32 (reference lib/ggml.c:6414-6520)
+                // W (+)= f32 or f16 matrix: the LoRA merge, ggml_compute_forward_add_q_f32 (reference lib/ggml.c:6414-6520) or, for a
+                // cached f16 adapter, ggml_compute_forward_add_q_f16 (:12372-12483)
                 const ggml_tensor *a = node->src0, *b = node->src1;
-                need_f32(b, "add (quantised + f32) src1");
+                if (b->type != GGML_TYPE_F32 && b->type != GGML_TYPE_F16)
+                    B200_FAIL("add (quantised + %s): src1 type is not supported by the B200 backend (f32, f16)", k_tname[b->type]);
                 B200_ASSERT(node->type == a->type && same_shape(a, b) && same_shape(a, node) && a->ne[2] == 1 && a->ne[3] == 1);
-                B200_ASSERT(a->nb[0] == k_tsize[a->type] && b->nb[0] == sizeof(float) && node->nb[0] == k_tsize[a->type] && a->ne[0] % 32 == 0);
-                FLC(fl_dev_add_q_f32((int)a->type, weight_ptr(a, cctx), a->nb[1], (int)a->ne[1], (int)a->ne[0],
-                                     (const float *)dev_ptr(b->data, nbytes_of(b), cctx), b->nb[1] / sizeof(float), dev_ptr(node->data, nbytes_of(node), cctx), node->nb[1]));
+                B200_ASSERT(a->nb[0] == k_tsize[a->type] && b->nb[0] == k_tsize[b->type] && node->nb[0] == k_tsize[a->type] && a->ne[0] % 32 == 0);
+                // use_mmap: the reference merges into a heap copy of the mapped weights (reference lib/llama.cpp:864-870).  The copy of an
+                // earlier attach, since detached and freed, may have lain on the same addresses, and its device mirror still holds that
+                // copy's merged bytes: start again from the host bytes.
+                const int mi = find_mirror(a->data);
+                if (mi >= 0 && g_mirrors[mi].kind == MK_EXTERNAL && !g_mirrors[mi].shared) {
+                    FLC(fl_sync());
+                    forget(g_mirrors[mi]);
+                    g_last_mirror = -1;
+                }
+                const void *X = dev_ptr(b->data, nbytes_of(b), cctx);
+                void *D = dev_ptr(node->data, nbytes_of(node), cctx);
+                if (b->type == GGML_TYPE_F32)
+                    FLC(fl_dev_add_q_f32((int)a->type, weight_ptr(a, cctx), a->nb[1], (int)a->ne[1], (int)a->ne[0], (const float *)X, b->nb[1] / 4, D, node->nb[1]));
+                else if (!fl_dev_add_q_f16)
+                    B200_FAIL("add (quantised + f16): the device layer has no fl_dev_add_q_f16");
+                else
+                    FLC(fl_dev_add_q_f16((int)a->type, weight_ptr(a, cctx), a->nb[1], (int)a->ne[1], (int)a->ne[0], (const uint16_t *)X, b->nb[1] / 2, D, node->nb[1]));
                 // the host tensor follows the device (tensor-parallel shards are uploaded from the HOST tensor, and a mirror that is
                 // dropped later would otherwise come back with the unmerged bytes)
                 FLC(fl_d2h(node->data, dev_ptr(node->data, nbytes_of(node), cctx), nbytes_of(node)));
@@ -1101,10 +1127,15 @@ void exec_node(ggml_tensor *node, const ggml_context *cctx) {
             exec_mul_mat(node, cctx);
             return;
         case GGML_OP_SCALE: {
-            need_f32(node->src0, "scale");
+            // f16: the detach of a cached f16 adapter, ggml_compute_forward_scale_f16 (reference lib/ggml.c:12485-12524)
+            if (node->src0->type != GGML_TYPE_F16) need_f32(node->src0, "scale");
             if (node->src1->op != GGML_OP_NONE) B200_FAIL("scale: the factor must be a host constant (ggml_new_f32)");
             fl_view d = view_of(node, cctx);
-            FLC(fl_dev_scale(&d, *(const float *)node->src1->data));
+            if (node->src0->type == GGML_TYPE_F16) {
+                if (!fl_dev_scale_f16) B200_FAIL("scale (f16): the device layer has no fl_dev_scale_f16");
+                FLC(fl_dev_scale_f16(&d, *(const float *)node->src1->data));
+            }
+            else FLC(fl_dev_scale(&d, *(const float *)node->src1->data));
             return;
         }
         case GGML_OP_DIAG_MASK_INF: {
@@ -1327,6 +1358,7 @@ static void packed_shards_clear() {
     for (auto &kv : g_packed) fl_dev_free(kv.second.dev);
     g_packed.clear();
     g_shard_bytes = 0;
+    g_tp_realign = true;
 }
 namespace {
 // device copy of (kind SH_FULL) the whole tensor, (SH_ROWS) rows [a, a + b), (SH_COLS) blocks [a, a + b) of every row with row stride *stride_out
@@ -1787,6 +1819,7 @@ DecodeState *run_decode_plan(const ggml_context *ctx, ggml_cgraph *g, DecodeOutp
             // token kernel's polls for the other ranks' vector elements give up after 2 s: line the ranks up first (one tiny collective).
             FLC(fl_comm_allreduce_f32(D.ws.m3, 1));
             FLC(fl_sync());
+            g_tp_realign = false;
         }
         if (!D.no_token_plan) {
             // one eager pass first: sets kernel attributes, and gives this token's result
@@ -1806,6 +1839,11 @@ DecodeState *run_decode_plan(const ggml_context *ctx, ggml_cgraph *g, DecodeOutp
         }
     }
     if (D.no_token_plan) return nullptr;        // node by node
+    if (P.world > 1 && g_tp_realign) {
+        FLC(fl_comm_allreduce_f32(D.ws.m3, 1));
+        FLC(fl_sync());
+        g_tp_realign = false;
+    }
     if (eager) {
         FLC(fl_event_record(ev0));
         if (D.token_plan) issue_decode_token_kernel(P, D.token_plan); else issue_decode(P, S.d_npast);

@@ -120,10 +120,15 @@ int fl_dev_quantize_q4_file(int type, int src_type, const void *x_dev, void *y_d
  * fl_dev_quantize_q4_simd: device-resident fl_quantize_rows_q4_simd.
  * fl_dev_add_q_f32: ggml_compute_forward_add_q_f32 (lib/ggml.c:6414-6520): row r of dst = quantize_row_q(dequantize_row_q(row r of W) +
  *   row r of X); dst may be W itself (ggml_add_inplace).  Bit-exact.
+ * fl_dev_add_q_f16: ggml_compute_forward_add_q_f16 (lib/ggml.c:12372-12483), the merge of a cached f16 adapter: fl_dev_add_q_f32 with X
+ *   as f16 bits, each element widened exactly to fp32 before the one fp32 add.  Bit-exact.
+ * fl_dev_scale_f16: ggml_compute_forward_scale_f16 (:12485-12524), in place on a contiguous f16 tensor: x = fp16_rn(fp32(x) * v).
  * fl_dev_mul_mat_f32_ref: ggml_mul_mat of two f32 matrices with ggml_vec_dot_f32's summation order of the AVX2 + FMA build
  *   (lib/ggml.c:2295-2325): out[j * ldo + i] = dot(A row i, B row j), K elements.  Bit-exact; meant for small K (B*A of a LoRA adapter). */
 int fl_dev_quantize_q4_simd(int type, const float *x, void *y, int k, int nrows);
 int fl_dev_add_q_f32(int type, const void *W, size_t w_row_stride_bytes, int M, int K, const float *X, size_t x_row_stride_elems, void *dst,
+                     size_t dst_row_stride_bytes);
+int fl_dev_add_q_f16(int type, const void *W, size_t w_row_stride_bytes, int M, int K, const uint16_t *X, size_t x_row_stride_elems, void *dst,
                      size_t dst_row_stride_bytes);
 int fl_dev_mul_mat_f32_ref(const float *A, size_t lda_elems, int Ma, const float *B, size_t ldb_elems, int Mb, int K, float *out, size_t ldo_elems);
 
@@ -154,6 +159,7 @@ int fl_dev_add(const fl_view *a, const fl_view *b, const fl_view *dst);
 int fl_dev_mul(const fl_view *a, const fl_view *b, const fl_view *dst);
 int fl_dev_repeat(const fl_view *src, const fl_view *dst);
 int fl_dev_scale(const fl_view *t, float v);                                /* in place */
+int fl_dev_scale_f16(const fl_view *t, float v);                            /* in place, contiguous f16 (fl_dev_add_q_f16 above) */
 int fl_dev_silu(const fl_view *src, const fl_view *dst);                    /* fp16-table silu (lib/ggml.c:3207-3215) */
 int fl_dev_diag_mask_inf(const fl_view *t, int n_past);                     /* in place */
 int fl_dev_soft_max(const fl_view *t);                                      /* in place, fp16-table exp */
