@@ -90,6 +90,11 @@ __device__ __forceinline__ void fl_mbar_wait(uint32_t bar, uint32_t parity) {
     while (!fl_mbar_try_wait(bar, parity)) {
     }
 }
+// bounded mbarrier wait: a protocol bug traps (the launch fails with an error) instead of hanging the GPU
+__device__ __forceinline__ void fl_mbar_wait_bounded(uint32_t bar, uint32_t parity) {
+    for (uint32_t n = 0; !fl_mbar_try_wait(bar, parity); n++)
+        if (n > (1u << 24)) asm volatile("trap;");
+}
 
 // 1-D bulk async copy global -> shared through the TMA unit (SASS: UBLKCP.S.G); completion is
 // signalled on `bar` as `bytes` transaction bytes.  dst/src 16-B aligned, bytes % 16 == 0.

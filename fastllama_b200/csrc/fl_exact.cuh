@@ -30,15 +30,25 @@ static_assert(sizeof(fl_yx) == 80, "prepared activation block");
 #ifdef __CUDACC__
 __device__ __forceinline__ uint32_t fx_bias(uint32_t y4, int off) { return (uint32_t)(FX_MAGIC_I - off * fl_dp4a_ss(0x01010101u, y4, 0)); }
 
-// w: the 4 weight bytes (8 nibbles) of this lane; d = dx * dy already rounded; y: this lane's entry of the prepared block
-__device__ __forceinline__ void fx_block(uint32_t w, float d, const uint4 y, float &a0, float &a1) {
+// w: the 4 weight bytes (8 nibbles) of this lane -> its elements 0,1,2,3 (wa) and 4,5,6,7 (wb) as unsigned bytes
+__device__ __forceinline__ void fx_split(uint32_t w, uint32_t &wa, uint32_t &wb) {
     const uint32_t lo = w & 0x0F0F0F0Fu, hi = (w >> 4) & 0x0F0F0F0Fu;      // elements 0,2,4,6 | 1,3,5,7
-    const uint32_t wa = __byte_perm(lo, hi, 0x5140);                         // elements 0,1,2,3
-    const uint32_t wb = __byte_perm(lo, hi, 0x7362);                         // elements 4,5,6,7
+    wa = __byte_perm(lo, hi, 0x5140);                                        // elements 0,1,2,3
+    wb = __byte_perm(lo, hi, 0x7362);                                        // elements 4,5,6,7
+}
+// wa, wb: fx_split of the lane's weight word (split once, used against any number of activation columns);
+// d = dx * dy already rounded; y: this lane's entry of the prepared block
+__device__ __forceinline__ void fx_block_split(uint32_t wa, uint32_t wb, float d, const uint4 y, float &a0, float &a1) {
     const float qa = __fsub_rn(__int_as_float(fl_dp4a_us(wa, y.x, (int)y.z)), FX_MAGIC_F);    // |sum| <= 4 * 15 * 128 < 2^22: exact
     const float qb = __fsub_rn(__int_as_float(fl_dp4a_us(wb, y.y, (int)y.w)), FX_MAGIC_F);
     a0 = __fmaf_rn(d, qa, a0);
     a1 = __fmaf_rn(d, qb, a1);
+}
+// w: the 4 weight bytes (8 nibbles) of this lane; d = dx * dy already rounded; y: this lane's entry of the prepared block
+__device__ __forceinline__ void fx_block(uint32_t w, float d, const uint4 y, float &a0, float &a1) {
+    uint32_t wa, wb;
+    fx_split(w, wa, wb);
+    fx_block_split(wa, wb, d, y, a0, a1);
 }
 // the reference's lane reduction; lanes 4r .. 4r+3 hold (a[2jj], a[2jj+1]); the row total is valid in lane 4r
 __device__ __forceinline__ float fx_reduce(float a0, float a1) {

@@ -66,5 +66,9 @@ int flk_mul_mat_f32_ref(cudaStream_t st, const float *A, size_t lda, int Ma, con
 // fl_exact_kernels.cu: results with the reference's fp32 bits (fl_exact.cuh): q4 x q8_0 matmul for any M, K, N, and the f32 mul_mat
 int flk_mul_mat_q_ref(cudaStream_t st, int type, const void *W, size_t w_row_stride, int M, int K, const void *Yq8, int N, float *dst,
                       size_t dst_row_stride);
+// the same bits as a tiled GEMM (shared-memory ring, TMA) for multi-token evals; operands: q4_0 / q4_1, 16-byte aligned W and rows
+int flk_mul_mat_q_ref_tiled_supported(int type, const void *W, size_t w_row_stride, int M, int K, int N);
+int flk_mul_mat_q_ref_tiled(cudaStream_t st, int type, const void *W, size_t w_row_stride, int M, int K, const void *Yq8, int N, float *dst,
+                            size_t dst_row_stride);
 int flk_mul_mat_f32_ref4(cudaStream_t st, const fl_view &a, const fl_view &b, const fl_view &d);
 void flk_exact_release();

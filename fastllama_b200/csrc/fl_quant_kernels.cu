@@ -623,6 +623,9 @@ static int launch_ring(cudaStream_t st, int type, int nfull, fl_ring_params &p, 
     return 0;
 }
 
+// Fewest activation columns for which the tiled reference-order kernel beats k_mul_mat_q_ref (tools/time_exact_ingest.py).
+#define FL_REF_TILED_MIN_N 8
+
 int flk_mul_mat_q(cudaStream_t st, int type, const void *W, size_t wrs, int M, int K, const void *Yq8, int N,
                   float *dst, size_t drs, int impl) {
     FL_REQUIRE(type == FL_TYPE_Q4_0 || type == FL_TYPE_Q4_1, "mul_mat_q: unsupported weight type %d", type);
@@ -632,16 +635,20 @@ int flk_mul_mat_q(cudaStream_t st, int type, const void *W, size_t wrs, int M, i
     // impl 0 (what the graph executor passes): results carry the reference's bits -- the reference-order kernel of fl_exact_kernels.cu --
     // except for multi-token evals of N >= 16 columns, which go to the wgmma GEMM (same per-block arithmetic, block terms added in
     // another fp32 order: within the stated budget, not bit-identical) unless FASTLLAMA_B200_INGEST=exact.
+    // The reference-order results come from the tiled kernel from FL_REF_TILED_MIN_N columns on, when its TMA copies take the operands
+    // (16-byte aligned rows), and from the warp-per-8-rows kernel otherwise: the same arithmetic, the same bits.
     // The other kernels stay selectable for measurements and their own tests: 1 plain, 2 TMA ring matvec, 3 mma.sync,
-    // 4-7 wgmma (column tile chosen / 32 / 64 / 64), 8 reference order.
+    // 4-7 wgmma (column tile chosen / 32 / 64 / 64), 8 reference order (k_mul_mat_q_ref), 9 reference order tiled (k_mul_mat_q_ref_tiled).
     if (impl == 0) {
         static const int umma_auto = getenv("FASTLLAMA_B200_UMMA") ? atoi(getenv("FASTLLAMA_B200_UMMA")) : 1;     // FASTLLAMA_B200_UMMA=0: no tensor-core path
         const char *ing = getenv("FASTLLAMA_B200_INGEST");               // read per call: tests and callers may switch it between evals
         const bool exact_ingest = ing && !strcmp(ing, "exact");
         if (umma_auto && !exact_ingest && N >= 16 && flk_mul_mat_q_umma_supported(type, W, wrs, M, K, N)) return flk_mul_mat_q_umma(st, type, W, wrs, M, K, Yq8, N, dst, drs, 0);
+        if (N >= FL_REF_TILED_MIN_N && flk_mul_mat_q_ref_tiled_supported(type, W, wrs, M, K, N)) return flk_mul_mat_q_ref_tiled(st, type, W, wrs, M, K, Yq8, N, dst, drs);
         return flk_mul_mat_q_ref(st, type, W, wrs, M, K, Yq8, N, dst, drs);
     }
     if (impl == 8) return flk_mul_mat_q_ref(st, type, W, wrs, M, K, Yq8, N, dst, drs);
+    if (impl == 9) return flk_mul_mat_q_ref_tiled(st, type, W, wrs, M, K, Yq8, N, dst, drs);
     if (impl >= 4 && impl <= 7) return flk_mul_mat_q_umma(st, type, W, wrs, M, K, Yq8, N, dst, drs, impl == 4 ? 0 : 16 << (impl - 4));
     if (impl == 3) return flk_mul_mat_q_mma(st, type, W, wrs, M, K, Yq8, N, dst, drs);
     if (impl == 2) {

@@ -27,6 +27,7 @@
 
 #include "fl_common.cuh"
 #include "fl_kernels.h"
+#include "fl_tma.cuh"
 
 #define UM_M 64               // weight rows per CTA = the M of one wgmma
 #define UM_KC 4               // k-blocks per TMA stage
@@ -34,20 +35,10 @@
 #define UM_THREADS (4 * 32 + 32)
 
 // ---- PTX wrappers --------------------------------------------------------------------------------
-__device__ __forceinline__ void um_tma_2d(uint32_t dst, const CUtensorMap *tm, int c0, int c1, uint32_t bar) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst), "l"(tm), "r"(c0),
-                 "r"(c1), "r"(bar)
-                 : "memory");
-}
 // K-major operand, no swizzle: core matrix = 8 rows x 16 bytes, contiguous (128 B); LBO = byte distance between the two
 // 16-byte K halves, SBO = byte distance between 8-row groups (wgmma matrix descriptor, swizzle mode 0)
 __device__ __forceinline__ uint64_t um_smem_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32);
-}
-// bounded mbarrier wait: a protocol bug traps (the launch fails with an error) instead of hanging the GPU
-__device__ __forceinline__ void um_wait(uint32_t bar, uint32_t parity) {
-    for (uint32_t n = 0; !fl_mbar_try_wait(bar, parity); n++)
-        if (n > (1u << 24)) asm volatile("trap;");
 }
 __device__ __forceinline__ void um_wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void um_wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -191,7 +182,7 @@ __global__ void __launch_bounds__(UM_THREADS) k_mul_mat_q_umma(const __grid_cons
 
         for (int st = 0; st < nstages; st++) {
             const int s = st % UM_STAGES;
-            um_wait(raw_full(s), (uint32_t)(st / UM_STAGES) & 1u);
+            fl_mbar_wait_bounded(raw_full(s), (uint32_t)(st / UM_STAGES) & 1u);
             const uint8_t *raw = smem + (size_t)s * L::STAGE;
             const uint32_t *wa = (const uint32_t *)(raw + (size_t)ra * (UM_KC * BB));
             const uint32_t *wb = (const uint32_t *)(raw + (size_t)rb * (UM_KC * BB));
@@ -265,11 +256,11 @@ __global__ void __launch_bounds__(UM_THREADS) k_mul_mat_q_umma(const __grid_cons
         const float *sy = prm.sy + (size_t)tile_n * nbp * NT;
         for (int st = 0; st < nstages; st++) {
             const int s = st % UM_STAGES;
-            um_wait(raw_empty(s), ((uint32_t)(st / UM_STAGES) & 1u) ^ 1u);
+            fl_mbar_wait_bounded(raw_empty(s), ((uint32_t)(st / UM_STAGES) & 1u) ^ 1u);
             const uint32_t dst = sm0 + (uint32_t)(s * L::STAGE);
             const int kb0 = st * UM_KC;
             fl_mbar_expect_tx(raw_full(s), (uint32_t)L::STAGE);
-            um_tma_2d(dst, &tmap_w, kb0 * (BB / 4), m0, raw_full(s));                                   // 64 rows x KC blocks of raw q4
+            fl_tma_2d(dst, &tmap_w, kb0 * (BB / 4), m0, raw_full(s));                                   // 64 rows x KC blocks of raw q4
             fl_bulk_g2s(dst + L::RAW_A, yq + (size_t)kb0 * (NT * 32), (uint32_t)L::RAW_B, raw_full(s));
             fl_bulk_g2s(dst + L::RAW_A + L::RAW_B, dy + (size_t)kb0 * NT, (uint32_t)L::RAW_S, raw_full(s));
             if (TYPE == FL_TYPE_Q4_1) fl_bulk_g2s(dst + L::RAW_A + L::RAW_B + L::RAW_S, sy + (size_t)kb0 * NT, (uint32_t)L::RAW_S, raw_full(s));
@@ -278,18 +269,6 @@ __global__ void __launch_bounds__(UM_THREADS) k_mul_mat_q_umma(const __grid_cons
 }
 
 // ---- host ------------------------------------------------------------------------------------------
-typedef CUresult (*um_encode_fn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
-                                 const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static um_encode_fn um_get_encode() {
-    static um_encode_fn fn = nullptr;
-    if (!fn) {
-        void *p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess) fn = (um_encode_fn)p;
-    }
-    return fn;
-}
-
 static struct {
     uint8_t *yq = nullptr;
     float *dy = nullptr, *sy = nullptr;
@@ -299,7 +278,7 @@ static struct {
 int flk_mul_mat_q_umma_supported(int type, const void *W, size_t wrs, int M, int K, int N) {
     if (type != FL_TYPE_Q4_0 && type != FL_TYPE_Q4_1) return 0;
     if (((uintptr_t)W & 15) != 0 || (wrs & 15) != 0 || K % 32 != 0 || M < 1 || N < 1) return 0;
-    return um_get_encode() != nullptr;
+    return fl_tma_get_encode() != nullptr;
 }
 
 template <int TYPE, int NT>
@@ -323,7 +302,7 @@ static int um_launch(cudaStream_t st, const void *W, size_t wrs, int M, int K, c
     const cuuint64_t gstr[1] = {(cuuint64_t)wrs};
     const cuuint32_t box[2] = {(cuuint32_t)(UM_KC * L::BB / 4), (cuuint32_t)UM_M};
     const cuuint32_t estr[2] = {1, 1};
-    const CUresult cr = um_get_encode()(&tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, (void *)W, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    const CUresult cr = fl_tma_get_encode()(&tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, (void *)W, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                         CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     FL_REQUIRE(cr == CUDA_SUCCESS, "mul_mat_q (wgmma): cuTensorMapEncodeTiled failed (%d) for M=%d K=%d stride=%zu", (int)cr, M, K, wrs);
     static bool attr_done = false;

@@ -100,7 +100,9 @@ int fl_dev_quantize_q8_0(const float *x, size_t x_row_stride_bytes, void *y, int
  * else plain), 1 = plain warp-per-row LDG kernel, 2 = TMA-bulk-staged persistent matvec (N = 1 only), 3 = legacy tensor-core kernel
  * (mma.sync m16n8k32 u8 x s8 block sums, fp32 scales; any N), 4 = wgmma GEMM (fl_umma_kernel.cu: one wgmma M = 64,
  * K = 32 with 8-bit operands per quant block into registers, weights by TMA, exact fp32 block scaling; needs 16-byte aligned W rows),
- * 5 / 6 / 7 = the same with the column tile forced to 32 / 64 / 64. */
+ * 5 / 6 / 7 = the same with the column tile forced to 32 / 64 / 64, 8 = reference-order kernel (the reference's fp32 order and bits;
+ * any N, 4-byte aligned W rows), 9 = the same arithmetic as a shared-memory-tiled GEMM (k_mul_mat_q_ref_tiled; any N, needs 16-byte
+ * aligned W and row stride, else an error).  Impl 0 uses 9 for 8..15 columns and, under FASTLLAMA_B200_INGEST=exact, for every N >= 8. */
 int fl_dev_mul_mat_q(int type, const void *W, size_t w_row_stride_bytes, int M, int K, const void *Yq8, int N,
                      float *dst, size_t dst_row_stride_elems, int impl);
 
