@@ -47,6 +47,8 @@ int flk_cpy_f32(cudaStream_t st, const fl_view &src, const fl_view &dst);
 int flk_mul_mat_f32(cudaStream_t st, const fl_view &src0, const fl_view &src1, const fl_view &dst);
 // [world][N][n_local] (an all-gather's output) -> [N][world * n_local], + residual [N][world * n_local] when it is not null
 int flk_tp_unshard(cudaStream_t st, const float *gathered, int world, int N, int n_local, const float *residual, float *dst);
+int flk_tp_unshard_v(cudaStream_t st, const float *gathered, int world, int N, int stride, const int *first, const int *count, const float *residual,
+                     float *dst);
 
 // fl_umma_kernel.cu: N > 1 on the Hopper tensor cores: one wgmma (M = 64, K = 32, 8-bit operands) per quant block into registers,
 // weights by TMA, exact fp32 block scaling by the same warpgroup.  nt_hint: column-tile width (0 = choose; 32 / 64; 128 is taken as 64)

@@ -311,6 +311,73 @@ int flk_tp_unshard(cudaStream_t st, const float *gathered, int world, int N, int
 }
 
 // ------------------------------------------------------------------------------------------------
+// the same for uneven slices (tensor parallelism at a world size that does not divide the shape): rank r's [N][count_r] block
+// sits at g + r * N * stride (the all-gather of slices padded to `stride` floats) and goes to columns [first_r, first_r + count_r)
+// of [N][n], n = sum of the counts.  One thread per V consecutive elements of one rank's block row; the per-rank tables are
+// kernel parameters.  V = 4 for ranks whose count, first column and block start keep every float4 16-byte aligned (the caller
+// checks this per rank, k_vmask); the other ranks are covered by the V = 1 launch.  Each element is written by exactly one launch.
+// ------------------------------------------------------------------------------------------------
+struct tp_slices {
+    int first[8], count[8];
+    int64_t start[9];        // prefix sums of N * (count_r / V): thread i belongs to the rank r with start[r] <= i < start[r + 1]
+};
+template <int V>
+__global__ void k_tp_unshard_v(const float *__restrict__ g, int world, int N, int stride, int n, const tp_slices t, const float *res, float *dst) {
+    using T = typename std::conditional<V == 4, float4, float>::type;
+    const int64_t total = t.start[world];
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        int r = 0;
+        while (i >= t.start[r + 1]) r++;
+        const int cv = t.count[r] / V;
+        const int64_t k = i - t.start[r], col = k / cv;
+        const int j = (int)(k - col * cv) * V;
+        T v =*(const T *)(g + (int64_t)r * N * stride + col * t.count[r] + j);
+        const int64_t o = col * n + t.first[r] + j;
+        if (res) {
+            const T b = *(const T *)(res + o);
+            if constexpr (V == 4) { v.x = __fadd_rn(v.x, b.x); v.y = __fadd_rn(v.y, b.y); v.z = __fadd_rn(v.z, b.z); v.w = __fadd_rn(v.w, b.w); }
+            else v = __fadd_rn(v, b);
+        }
+        *(T *)(dst + o) = v;
+    }
+}
+int flk_tp_unshard_v(cudaStream_t st, const float *gathered, int world, int N, int stride, const int *first, const int *count, const float *residual,
+                     float *dst) {
+    FL_REQUIRE(gathered && dst && first && count && world >= 1 && world <= 8 && N >= 0 && stride >= 0, "tp_unshard_v: bad arguments");
+    int n = 0;
+    for (int r = 0; r < world; r++) {
+        FL_REQUIRE(count[r] >= 0 && count[r] <= stride && first[r] >= 0, "tp_unshard_v: rank %d has a bad slice (%d, %d)", r, first[r], count[r]);
+        n += count[r];
+    }
+    for (int r = 0; r < world; r++) FL_REQUIRE((int64_t)first[r] + count[r] <= n, "tp_unshard_v: rank %d's slice ends past the %d columns", r, n);
+    if ((int64_t)N * n == 0) return 0;
+    // float4 for a rank when its block rows and its output columns stay 16-byte aligned in every row
+    const bool base16 = (((uintptr_t)gathered | (uintptr_t)dst | (uintptr_t)residual) & 15) == 0;
+    tp_slices t4, t1;
+    t4.start[0] = t1.start[0] = 0;
+    for (int r = 0; r < world; r++) {
+        const bool vec = base16 && count[r] % 4 == 0 && first[r] % 4 == 0 && n % 4 == 0 && ((int64_t)r * N * stride) % 4 == 0;
+        t4.first[r] = t1.first[r] = first[r];
+        t4.count[r] = vec ? count[r] : 0;
+        t1.count[r] = vec ? 0 : count[r];
+        t4.start[r + 1] = t4.start[r] + (int64_t)N * (t4.count[r] / 4);
+        t1.start[r + 1] = t1.start[r] + (int64_t)N * t1.count[r];
+    }
+    for (int r = world; r < 8; r++) { t4.first[r] = t1.first[r] = 0; t4.count[r] = t1.count[r] = 0; t4.start[r + 1] = t4.start[world]; t1.start[r + 1] = t1.start[world]; }
+    if (t4.start[world] > 0) {
+        k_tp_unshard_v<4><<<ew_grid(t4.start[world], 256), 256, 0, st>>>(gathered, world, N, stride, n, t4, residual, dst);
+        fl_count_launch();
+        FL_CUDA_OK(cudaGetLastError());
+    }
+    if (t1.start[world] > 0) {
+        k_tp_unshard_v<1><<<ew_grid(t1.start[world], 256), 256, 0, st>>>(gathered, world, N, stride, n, t1, residual, dst);
+        fl_count_launch();
+        FL_CUDA_OK(cudaGetLastError());
+    }
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
 // mul_mat f32 x f32 (attention scores and weighted values of a multi-token eval): the reference-order kernel of
 // fl_exact_kernels.cu (one warp per output group, lane l = element l of ggml_vec_dot_f32's 32-float step).
 // ------------------------------------------------------------------------------------------------

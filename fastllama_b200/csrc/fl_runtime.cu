@@ -384,6 +384,11 @@ extern "C" int fl_dev_tp_unshard(const float *gathered, int world, int N, int n_
     FL_NEED_INIT();
     return flk_tp_unshard(g.stream, gathered, world, N, n_local, residual, dst);
 }
+extern "C" int fl_dev_tp_unshard_v(const float *gathered, int world, int N, int slice_stride, const int *first, const int *count, const float *residual,
+                                   float *dst) {
+    FL_NEED_INIT();
+    return flk_tp_unshard_v(g.stream, gathered, world, N, slice_stride, first, count, residual, dst);
+}
 
 // ---- fused decode step ------------------------------------------------------------------------
 extern "C" int fl_dev_mv_fused_supported(int type, int K, int mtot) { return flk_mv_fused_supported(type, K, mtot); }

@@ -35,6 +35,10 @@
 // Bound weakly, so that a device layer without it (one built before the tensor-parallel prompt plan, such as the CPU stand-in the
 // host-logic tests load) still loads: multi-token evals then keep the replicated executor (run_prompt_plan).  libfl_cuda.so exports it.
 extern "C" int fl_dev_tp_unshard(const float *gathered, int world, int N, int n_local, const float *residual, float *dst) __attribute__((weak));
+// Its uneven-slice form, bound weakly for the same reason: without it, worlds that divide the model's shapes run as before and the others
+// keep the replicated executor.
+extern "C" int fl_dev_tp_unshard_v(const float *gathered, int world, int N, int slice_stride, const int *first, const int *count, const float *residual,
+                                   float *dst) __attribute__((weak));
 // The f16 ops of a cached f16 LoRA adapter, bound weakly for the same reason: a device layer without them still loads and runs everything
 // else, and an f16 adapter on it fails with an error naming the missing entry point.  libfl_cuda.so exports both.
 extern "C" int fl_dev_add_q_f16(int type, const void *W, size_t w_row_stride_bytes, int M, int K, const uint16_t *X, size_t x_row_stride_elems,
@@ -1196,8 +1200,13 @@ struct DecodePlan {
     std::vector<LayerPlan> layers;
     fl_mv_args head;
     int world = 1, heads_local = 0;             // tensor-parallel degree and heads per rank
+    int embd_first = 0, ff_first = 0;           // where this rank's slices of n_embd (whole heads) and n_ff start (tp_partition)
     float *logits_local = nullptr, *logits_all = nullptr;
     int vocab_local = 0;
+    // uneven vocabulary slices: every rank's logits padded to vocab_stride floats are all-gathered into logits_gather, and
+    // fl_dev_tp_unshard_v compacts them into logits_all (vocab_stride 0: equal slices, gathered straight into logits_all)
+    float *logits_gather = nullptr;
+    int vocab_stride = 0, vocab_first[8] = {0}, vocab_count[8] = {0};
 };
 // Private device workspace of the decode step.  The compute arena cannot be used for intermediates:
 // its layout shifts from token to token (the K*Q score tensor grows with n_past), and the captured
@@ -1205,7 +1214,7 @@ struct DecodePlan {
 struct DecodeWs {
     int n_embd = 0, n_ff = 0, n_vocab = 0;
     float *xa = nullptr, *xb = nullptr, *q = nullptr, *att = nullptr, *ff = nullptr, *m1 = nullptr, *m3 = nullptr, *emb = nullptr, *logits = nullptr;
-    float *logits_local = nullptr;
+    float *logits_local = nullptr, *logits_gather = nullptr;
     int32_t *d_tok = nullptr;
     // The dataflow ("LL") vectors of the token kernel (include/fl_cuda.h, fl_mv_args): {value, epoch} words that hand the
     // activations from step to step without grid barriers.  Layout of the buffer: 4096 bytes of counters (word 0 = the running epoch),
@@ -1228,7 +1237,7 @@ struct DecodeState {
     bool no_token_plan = false;       // the current plan's graph is not one the token kernel takes: node-by-node execution
     bool tp_kv_sharded = false;   // tensor-parallel decode steps / prompt-plan evals have written only this rank's heads into the KV cache ...
     int tp_first_pos = 0, tp_end_pos = 0;   // ... for positions [tp_first_pos, tp_end_pos)
-    struct { int n_embd = 0, n_ctx = 0; std::vector<float *> k, v; } tp_kv;   // that cache on the device: every layer's K [pos][n_embd], V [n_embd][n_ctx]
+    struct { int n_embd = 0, n_ctx = 0, hd = 0; std::vector<float *> k, v; } tp_kv;   // that cache on the device: every layer's K [pos][n_embd], V [n_embd][n_ctx]
 };
 // What every context's decode steps share: evals run one at a time, so the step's scalars and result staging are needed once.
 struct DecodeShared {
@@ -1298,12 +1307,15 @@ void mv_base(fl_mv_args &a, int type, int K) {
 void ensure_ws(DecodeWs &w, int n_embd, int n_ff, int n_vocab) {
     if (w.xa && w.n_embd == n_embd && w.n_ff == n_ff && w.n_vocab == n_vocab) return;
     if (w.xa) { FLC(fl_sync()); FLC(fl_dev_free(w.xa)); }
-    const size_t total = (size_t)n_embd * 6 + (size_t)n_ff * 2 + (size_t)n_vocab * 2 + 64;
+    // logits, logits_local and logits_gather take n_vocab and then some: the odd last row of an LM head is computed as a row pair whose
+    // second value lands one past the slice, and the padded all-gather of uneven slices holds up to 2 * world - 1 floats more
+    const size_t vcap = ((size_t)n_vocab + 16 + 3) & ~(size_t)3;
+    const size_t total = (size_t)n_embd * 6 + (size_t)n_ff * 2 + vcap * 3 + 64;
     float *base = (float *)fl_dev_malloc(total * sizeof(float));
     if (!base) B200_FAIL("decode workspace: %s", fl_last_error());
     w.xa = base; w.xb = w.xa + n_embd; w.q = w.xb + n_embd; w.att = w.q + n_embd; w.ff = w.att + n_embd; w.emb = w.ff + n_embd;
-    w.m1 = w.emb + n_embd; w.m3 = w.m1 + n_ff; w.logits = w.m3 + n_ff; w.logits_local = w.logits + n_vocab;
-    w.d_tok = (int32_t *)(w.logits_local + n_vocab);
+    w.m1 = w.emb + n_embd; w.m3 = w.m1 + n_ff; w.logits = w.m3 + n_ff; w.logits_local = w.logits + vcap; w.logits_gather = w.logits_local + vcap;
+    w.d_tok = (int32_t *)(w.logits_gather + vcap);
     w.n_embd = n_embd; w.n_ff = n_ff; w.n_vocab = n_vocab;
     const int world = fl_comm_world(), rank = fl_comm_rank();
     if (world > 1) {
@@ -1346,7 +1358,7 @@ struct ShardKey {
     bool operator==(const ShardKey &o) const { return host == o.host && kind == o.kind && a == o.a && b == o.b; }
 };
 struct ShardKeyHash { size_t operator()(const ShardKey &k) const { return std::hash<const void *>()(k.host) ^ ((size_t)k.kind * 0x9E3779B97F4A7C15ull) ^ ((size_t)k.a << 20) ^ (size_t)k.b; } };
-enum { SH_FULL = 0, SH_ROWS = 1, SH_COLS = 2 };
+enum { SH_FULL = 0, SH_ROWS = 1, SH_COLS = 2, SH_TAIL = 3 };
 struct Shard { void *dev; size_t bytes; };
 std::unordered_map<ShardKey, Shard, ShardKeyHash> g_packed;
 char *g_shard_staging = nullptr;
@@ -1361,7 +1373,45 @@ static void packed_shards_clear() {
     g_tp_realign = true;
 }
 namespace {
-// device copy of (kind SH_FULL) the whole tensor, (SH_ROWS) rows [a, a + b), (SH_COLS) blocks [a, a + b) of every row with row stride *stride_out
+// ---- the tensor-parallel partition (DESIGN.md section 7): the one rule every row split of the decode plan, the prompt plan and the KV
+// gather follows.  `total` rows are cut into whole units of `unit` rows; the units go to the ranks in order, as evenly as possible, the
+// first (units % world) ranks taking one more, and the rows left over after the last whole unit (the single last row of an odd
+// vocabulary) go with the last rank.  Where unit * world divides total this is the plain total / world split.  A rank may get no rows:
+// the plans then decline (tp_partition).
+struct TpSplit { int first, rows; };
+TpSplit tp_split(int total, int unit, int world, int rank) {
+    const int units = total / unit, base = units / world, extra = units % world;
+    const int u0 = rank * base + std::min(rank, extra), nu = base + (rank < extra ? 1 : 0);
+    const int first = u0 * unit, end = rank == world - 1 ? total : (u0 + nu) * unit;
+    return TpSplit{first, end - first};
+}
+// every rank's slice of n_embd (whole heads: wq / wk / wv / wo / w2 rows, A, B, X, the KV cache), n_ff (32-row groups: w1 / w3 rows, H)
+// and n_vocab (row pairs, the last one single when n_vocab is odd: LM-head rows and logits)
+struct TpPart {
+    std::vector<TpSplit> e, f, v;
+    int max_e = 0, max_f = 0, max_v = 0;
+    bool ok = false;                        // every rank owns at least one head, one n_ff group and one vocabulary row
+    bool even = false;                      // every kind splits into equal slices (the n / world split: fl_dev_tp_unshard suffices)
+};
+TpPart tp_partition(int n_embd, int hd, int n_ff, int n_vocab, int world) {
+    TpPart T;
+    bool ok = world >= 1 && hd > 0 && n_embd % hd == 0, even = true;
+    for (int r = 0; r < world; r++) {
+        T.e.push_back(tp_split(n_embd, hd, world, r)); T.f.push_back(tp_split(n_ff, 32, world, r)); T.v.push_back(tp_split(n_vocab, 2, world, r));
+        ok = ok && T.e[r].rows > 0 && T.f[r].rows > 0 && T.v[r].rows > 0;
+        even = even && T.e[r].rows == T.e[0].rows && T.f[r].rows == T.f[0].rows && T.v[r].rows == T.v[0].rows;
+        T.max_e = std::max(T.max_e, T.e[r].rows); T.max_f = std::max(T.max_f, T.f[r].rows); T.max_v = std::max(T.max_v, T.v[r].rows);
+    }
+    T.ok = ok; T.even = even;
+    return T;
+}
+// the firsts and counts of one kind, as fl_dev_tp_unshard_v takes them
+void tp_tables(const std::vector<TpSplit> &s, int *first, int *count) {
+    for (size_t r = 0; r < s.size(); r++) { first[r] = s[r].first; count[r] = s[r].rows; }
+}
+
+// device copy of (kind SH_FULL) the whole tensor, (SH_ROWS) rows [a, a + b), (SH_COLS) blocks [a, a + b) of every row with row stride
+// *stride_out, (SH_TAIL) row a twice: the last row of an odd row count as the row pair the token kernel works in
 const void *tp_shard(const ggml_tensor *w, int kind, int a, int b, size_t *stride_out = nullptr) {
     const size_t bb = k_tsize[w->type];
     const size_t stride = kind == SH_COLS ? (((size_t)b * bb + 15) & ~(size_t)15) : w->nb[1];
@@ -1371,6 +1421,15 @@ const void *tp_shard(const ggml_tensor *w, int kind, int a, int b, size_t *strid
     if (it != g_packed.end()) return it->second.dev;
     ensure_backend();
     const size_t rows = (size_t)nrows(w);
+    if (kind == SH_TAIL) {
+        const size_t bytes = 2 * w->nb[1];
+        char *dst = (char *)fl_dev_malloc(bytes + 256);
+        if (!dst) B200_FAIL("last-row copy of %zu bytes: %s", bytes, fl_last_error());
+        for (int i = 0; i < 2; i++) FLC(fl_h2d(dst + i * w->nb[1], (const char *)w->data + (size_t)a * w->nb[1], w->nb[1]));
+        g_packed[key] = Shard{dst, bytes};
+        g_shard_bytes += bytes;
+        return dst;
+    }
     const size_t bytes = kind == SH_FULL ? nbytes_of(w) : kind == SH_ROWS ? (size_t)b * w->nb[1] : stride * rows;
     void *dst = fl_dev_malloc(bytes + 256);
     if (!dst) B200_FAIL("tensor-parallel shard of %zu bytes: %s", bytes, fl_last_error());
@@ -1540,9 +1599,18 @@ bool match_decode(const ggml_context *ctx, ggml_cgraph *g, DecodePlan &P, Decode
     EvalGraph E;
     if (!parse_eval_graph(g, E)) return false;
     PM(E.N == 1);
+    const int n_embd = E.n_embd, n_head = E.n_head, n_ctx = E.n_ctx, n_past = E.n_past, hd = E.hd, n_ff = E.n_ff;
+    // this rank's heads, n_ff groups and vocabulary rows (one GPU: all of them)
+    const TpPart T = tp_partition(n_embd, hd, n_ff, E.n_vocab, world);
+    PM(T.ok && world <= 8);
+    if (world > 1) {
+        PM(n_ff % 32 == 0);
+        for (int r = 0; r < world; r++) PM(T.e[r].rows % 32 == 0);
+        for (int r = 0; r < world; r++) PM(T.v[r].rows == T.v[0].rows || fl_dev_tp_unshard_v);     // uneven logits: fl_dev_tp_unshard_v compacts them
+    }
+    const int e0 = T.e[rank].first, nl = T.e[rank].rows, f0 = T.f[rank].first, fl = T.f[rank].rows, v0 = T.v[rank].first, vl = T.v[rank].rows;
     D = &state_for(arena_of(E.layers[0].Kv->data), ctx);
     DecodeWs &W = D->ws;
-    const int n_embd = E.n_embd, n_head = E.n_head, n_ctx = E.n_ctx, n_past = E.n_past, hd = E.hd, n_ff = E.n_ff;
     ggml_tensor *n0 = E.emb;
     P.n_embd = n_embd;
     P.n_layer = E.n_layer;
@@ -1558,8 +1626,6 @@ bool match_decode(const ggml_context *ctx, ggml_cgraph *g, DecodePlan &P, Decode
         const ggml_tensor *wq = Ln.mq->src0, *wk = Ln.mk->src0, *wv = Ln.mv->src0, *wo = Ln.mo->src0, *w1 = Ln.m1->src0, *w3 = Ln.m3->src0, *w2 = Ln.m2->src0;
         PM(fl_dev_mv_fused_supported((int)wq->type, n_embd, 3 * n_embd) && fl_dev_mv_fused_supported((int)wo->type, n_embd, n_embd) &&
            fl_dev_mv_fused_supported((int)w1->type, n_embd, 2 * n_ff) && fl_dev_mv_fused_supported((int)w2->type, n_ff, n_embd));
-
-        if (world > 1) PM(n_head % world == 0 && n_ff % (32 * world) == 0 && (n_embd / world) % 32 == 0 && E.n_vocab % (2 * world) == 0);
         if (il == 0) {
             ensure_ws(W, n_embd, n_ff, E.n_vocab);
             P.emb_ids = W.d_tok; P.emb_dst = W.xa;
@@ -1574,8 +1640,7 @@ bool match_decode(const ggml_context *ctx, ggml_cgraph *g, DecodePlan &P, Decode
         // wq|wk|wv: rms_norm prologue, rope + cache-store epilogue
         mv_base(L.qkv, (int)wq->type, n_embd);
         L.qkv.nseg = 3;
-        const int nl_rows = n_embd / world;                              // this rank's rows of wq / wk / wv (whole heads)
-        L.qkv.seg_w[0] = wrows(wq, rank * nl_rows, nl_rows); L.qkv.seg_w[1] = wrows(wk, rank * nl_rows, nl_rows); L.qkv.seg_w[2] = wrows(wv, rank * nl_rows, nl_rows);
+        L.qkv.seg_w[0] = wrows(wq, e0, nl); L.qkv.seg_w[1] = wrows(wk, e0, nl); L.qkv.seg_w[2] = wrows(wv, e0, nl);   // this rank's heads
         L.qkv.seg_rows[0] = L.qkv.seg_rows[1] = L.qkv.seg_rows[2] = n_embd;
         L.qkv.seg_dst[0] = (float *)L.q;
         L.qkv.pro = FL_PRO_RMSNORM; L.qkv.x = xin; L.qkv.gamma = (const float *)wfull(Ln.attn_norm);
@@ -1587,8 +1652,7 @@ bool match_decode(const ggml_context *ctx, ggml_cgraph *g, DecodePlan &P, Decode
         L.wo.pro = FL_PRO_PLAIN; L.wo.x = L.att; L.wo.epi = FL_EPI_RESADD; L.wo.res = xin;
         // w1|w3: rms_norm prologue
         mv_base(L.w13, (int)w1->type, n_embd);
-        const int fl_rows = n_ff / world;
-        L.w13.nseg = 2; L.w13.seg_w[0] = wrows(w1, rank * fl_rows, fl_rows); L.w13.seg_w[1] = wrows(w3, rank * fl_rows, fl_rows);
+        L.w13.nseg = 2; L.w13.seg_w[0] = wrows(w1, f0, fl); L.w13.seg_w[1] = wrows(w3, f0, fl);
         L.w13.seg_rows[0] = L.w13.seg_rows[1] = n_ff; L.w13.seg_dst[0] = W.m1; L.w13.seg_dst[1] = W.m3;
         L.w13.pro = FL_PRO_RMSNORM; L.w13.x = W.ff; L.w13.gamma = (const float *)wfull(Ln.ffn_norm); L.w13.epi = FL_EPI_STORE;
         // w2: silu*mul prologue, residual epilogue
@@ -1599,29 +1663,42 @@ bool match_decode(const ggml_context *ctx, ggml_cgraph *g, DecodePlan &P, Decode
             // ---- tensor-parallel wiring (SURVEY.md 8e): EVERY matrix is row-split -- wq/wk/wv by heads, w1/w3 by n_ff slices, wo/w2 and
             // the output matrix by output rows -- and every activation vector is all-gathered as a dataflow (LL) vector (make_token_plan).
             // No K-split: a row is always summed over the whole K on one GPU, in the reference's order, so N GPUs produce the bits of one.
-            const int nl = n_embd / world, fl = n_ff / world;
-            L.kcache += (size_t)rank * nl; L.vcache += (size_t)rank * nl * n_ctx;   // this rank's heads
+            // Which rank owns which rows is tp_partition's: uneven slices change where a row is computed, never how.
+            L.kcache += (size_t)e0; L.vcache += (size_t)e0 * n_ctx;                     // this rank's heads
             for (int i = 0; i < 3; i++) L.qkv.seg_rows[i] = nl;                         // seg_w[] already point at this rank's rows (wrows)
             L.qkv.kcache = (float *)L.kcache; L.qkv.vcache = (float *)L.vcache;
-            L.wo.seg_w[0] = wrows(wo, rank * nl, nl); L.wo.seg_rows[0] = nl;
+            L.wo.seg_w[0] = wrows(wo, e0, nl); L.wo.seg_rows[0] = nl;
             L.w13.seg_rows[0] = L.w13.seg_rows[1] = fl;
-            L.w2.seg_w[0] = wrows(w2, rank * nl, nl); L.w2.seg_rows[0] = nl;
+            L.w2.seg_w[0] = wrows(w2, e0, nl); L.w2.seg_rows[0] = nl;
         }
         std::swap(xin, xout);
     }
     ggml_tensor *f = E.f, *lg = E.lg;
-    PM(lg->src0->ne[1] % 2 == 0 && fl_dev_mv_fused_supported((int)lg->src0->type, n_embd, (int)lg->src0->ne[1]));
+    // The token kernel works in row pairs: an odd slice (the last rank's when n_vocab is odd, on any number of GPUs) runs its even part
+    // as segment 0 and its last row as segment 1, a copy of that row twice (SH_TAIL) whose second value lands one past the slice
+    // (the workspace leaves room).  Same step, same arithmetic as every other LM-head row.
+    const int v_even = vl & ~1;
+    PM(fl_dev_mv_fused_supported((int)lg->src0->type, n_embd, vl + (vl & 1)));
     mv_base(P.head, (int)lg->src0->type, n_embd);
-    P.head.nseg = 1; P.head.seg_w[0] = wrows(lg->src0, rank * (int)(lg->src0->ne[1] / world), (int)(lg->src0->ne[1] / world)); P.head.seg_rows[0] = (int)lg->src0->ne[1]; P.head.seg_dst[0] = W.logits;
+    P.head.nseg = 1; P.head.seg_w[0] = wrows(lg->src0, v0, vl); P.head.seg_rows[0] = vl; P.head.seg_dst[0] = W.logits;
     PM(W.n_vocab == (int)lg->src0->ne[1] && is_vec(lg, W.n_vocab) && is_vec(f, n_embd));
     P.head.pro = FL_PRO_RMSNORM; P.head.x = xin; P.head.gamma = (const float *)wfull(E.out_norm); P.head.normed_out = W.emb;
     O.logits_host = lg->data; O.logits_bytes = (size_t)W.n_vocab * 4; O.emb_host = f->data; O.emb_bytes = (size_t)n_embd * 4;
-    P.world = world; P.heads_local = n_head / world;
+    P.world = world; P.heads_local = nl / hd;
+    P.embd_first = e0; P.ff_first = f0;
     if (world > 1) {
-        PM(W.n_vocab % (2 * world) == 0);
-        const int vl = W.n_vocab / world;
-        P.head.seg_rows[0] = vl; P.head.seg_dst[0] = W.logits_local;                 // seg_w[0] already points at this rank's rows
+        P.head.seg_dst[0] = W.logits_local;                                           // seg_w[0] already points at this rank's rows
         P.vocab_local = vl; P.logits_local = W.logits_local; P.logits_all = W.logits;
+        if (std::any_of(T.v.begin(), T.v.end(), [&](const TpSplit &s) { return s.rows != T.v[0].rows; })) {
+            P.vocab_stride = T.max_v; P.logits_gather = W.logits_gather;
+            tp_tables(T.v, P.vocab_first, P.vocab_count);
+        }
+    }
+    if (vl & 1) {
+        if (v_even == 0) P.head.nseg = 0;
+        else P.head.seg_rows[0] = v_even;
+        const int t = P.head.nseg++;
+        P.head.seg_w[t] = tp_shard(lg->src0, SH_TAIL, v0 + vl - 1, 1); P.head.seg_rows[t] = 2; P.head.seg_dst[t] = P.head.seg_dst[0] + v_even;
     }
     P.head.epi = FL_EPI_STORE;
     P.n_head = n_head; P.n_ctx = n_ctx; P.n_past = n_past;
@@ -1695,7 +1772,8 @@ void *make_token_plan(const DecodePlan &P, const DecodeWs &W, const int *d_npast
     static const bool dataflow_env = getenv("FASTLLAMA_B200_DATAFLOW") != nullptr;
     const int ll = (world > 1 || dataflow_env) ? 1 : 0;
     const size_t es = ll ? 2 : 1;                                   // floats per element
-    const int E = P.n_embd, F = W.n_ff, nl = E / world, fl = F / world, hd = E / P.n_head;
+    const int E = P.n_embd, F = W.n_ff, hd = E / P.n_head;
+    const size_t e0 = (size_t)P.embd_first, f0 = (size_t)P.ff_first;      // this rank's slices of the vectors (tp_partition)
     // element `first` of vector v (0 X, 1 A, 2 B, 3 H) in rank q's buffer, as mapped here
     auto vec = [&](int q, int v, size_t first) -> float * {
         const size_t off = 4096 + (size_t)(v < 3 ? v : 3) * W.ll_cap_embd * 8;
@@ -1717,37 +1795,37 @@ void *make_token_plan(const DecodePlan &P, const DecodeWs &W, const int *d_npast
         if (il == 0) s.mv.x = W.xa;
         else { s.mv.x = vec(rank, VX, 0); s.mv.x_ll = ll; s.mv.x_seq = seq0 - 1; }
         steps.push_back(s);
-        // attention over this rank's heads -> elements [rank * nl, +nl) of A (everywhere)
+        // attention over this rank's heads -> its elements [e0, +heads_local * hd) of A (everywhere)
         memset(&s, 0, sizeof(s));
         s.kind = 1; s.q = Lc.q; s.kcache = Lc.kcache; s.vcache = Lc.vcache; s.n_past = d_npast;
         s.k_row_stride = E; s.n_head = P.heads_local; s.head_dim = hd; s.n_ctx = P.n_ctx; s.scale = P.scale;
-        s.out = vec(rank, VA, (size_t)rank * nl); s.out_ll = ll; s.out_seq = seq0;
-        peers_of(VA, (size_t)rank * nl, s.out_peer, s.n_out_peer);
+        s.out = vec(rank, VA, e0); s.out_ll = ll; s.out_seq = seq0;
+        peers_of(VA, e0, s.out_peer, s.n_out_peer);
         steps.push_back(s);
-        // wo rows [rank * nl, +nl): B = wo . A + x
+        // wo, this rank's rows: B = wo . A + x
         memset(&s, 0, sizeof(s));
         s.kind = 0; s.mv = Lc.wo; s.mv.xadd = nullptr; s.mv.sum_out = nullptr; s.mv.row_stride_bytes = 0;
         s.mv.K = E; s.mv.pro = FL_PRO_PLAIN; s.mv.x = vec(rank, VA, 0); s.mv.x_ll = ll; s.mv.x_seq = seq0;
         s.mv.epi = FL_EPI_RESADD;
-        if (il == 0) { s.mv.res = W.xa + (size_t)rank * nl; s.mv.res_ll = 0; }
-        else { s.mv.res = vec(rank, VX, (size_t)rank * nl); s.mv.res_ll = ll; }
-        s.mv.seg_dst[0] = vec(rank, VB, (size_t)rank * nl); s.mv.out_ll = ll; s.mv.out_seq = seq0 + 1;
-        peers_of(VB, (size_t)rank * nl, s.mv.dst_peer, s.mv.n_dst_peer);
+        if (il == 0) { s.mv.res = W.xa + e0; s.mv.res_ll = 0; }
+        else { s.mv.res = vec(rank, VX, e0); s.mv.res_ll = ll; }
+        s.mv.seg_dst[0] = vec(rank, VB, e0); s.mv.out_ll = ll; s.mv.out_seq = seq0 + 1;
+        peers_of(VB, e0, s.mv.dst_peer, s.mv.n_dst_peer);
         steps.push_back(s);
-        // w1|w3 rows [rank * fl, +fl): H = silu(w1 . n) * (w3 . n), n = rms_norm(B) * gamma
+        // w1|w3, this rank's rows: H = silu(w1 . n) * (w3 . n), n = rms_norm(B) * gamma
         memset(&s, 0, sizeof(s));
         s.kind = 0; s.mv = Lc.w13; s.mv.xadd = nullptr; s.mv.sum_out = nullptr;
         s.mv.x = vec(rank, VB, 0); s.mv.x_ll = ll; s.mv.x_seq = seq0 + 1;
-        s.mv.swiglu = 1; s.mv.seg_dst[0] = vec(rank, VH, (size_t)rank * fl); s.mv.seg_dst[1] = nullptr; s.mv.out_ll = ll; s.mv.out_seq = seq0 + 2;
-        peers_of(VH, (size_t)rank * fl, s.mv.dst_peer, s.mv.n_dst_peer);
+        s.mv.swiglu = 1; s.mv.seg_dst[0] = vec(rank, VH, f0); s.mv.seg_dst[1] = nullptr; s.mv.out_ll = ll; s.mv.out_seq = seq0 + 2;
+        peers_of(VH, f0, s.mv.dst_peer, s.mv.n_dst_peer);
         steps.push_back(s);
-        // w2 rows [rank * nl, +nl): X = w2 . H + B
+        // w2, this rank's rows: X = w2 . H + B
         memset(&s, 0, sizeof(s));
         s.kind = 0; s.mv = Lc.w2; s.mv.xadd = nullptr; s.mv.sum_out = nullptr; s.mv.row_stride_bytes = 0;
         s.mv.K = F; s.mv.pro = FL_PRO_PLAIN; s.mv.b = nullptr; s.mv.x = vec(rank, VH, 0); s.mv.x_ll = ll; s.mv.x_seq = seq0 + 2;
-        s.mv.epi = FL_EPI_RESADD; s.mv.res = vec(rank, VB, (size_t)rank * nl); s.mv.res_ll = ll;
-        s.mv.seg_dst[0] = vec(rank, VX, (size_t)rank * nl); s.mv.out_ll = ll; s.mv.out_seq = seq0 + 3;
-        peers_of(VX, (size_t)rank * nl, s.mv.dst_peer, s.mv.n_dst_peer);
+        s.mv.epi = FL_EPI_RESADD; s.mv.res = vec(rank, VB, e0); s.mv.res_ll = ll;
+        s.mv.seg_dst[0] = vec(rank, VX, e0); s.mv.out_ll = ll; s.mv.out_seq = seq0 + 3;
+        peers_of(VX, e0, s.mv.dst_peer, s.mv.n_dst_peer);
         steps.push_back(s);
     }
     {
@@ -1767,7 +1845,12 @@ void *make_token_plan(const DecodePlan &P, const DecodeWs &W, const int *d_npast
 void issue_decode_token_kernel(const DecodePlan &P, void *token_plan) {
     FLC(fl_dev_dequantize_rows(P.emb_type, P.emb_w, P.emb_stride, P.emb_K, P.emb_ids, 1, P.emb_dst, (size_t)P.emb_K));
     FLC(fl_token_plan_launch(token_plan));
-    if (P.world > 1) FLC(fl_comm_allgather_f32(P.logits_local, P.logits_all, (size_t)P.vocab_local));
+    if (P.world > 1 && !P.vocab_stride) FLC(fl_comm_allgather_f32(P.logits_local, P.logits_all, (size_t)P.vocab_local));
+    if (P.world > 1 && P.vocab_stride) {
+        // uneven slices: NCCL gathers equal counts, so every rank sends its slice padded to the largest one, then one compaction
+        FLC(fl_comm_allgather_f32(P.logits_local, P.logits_gather, (size_t)P.vocab_stride));
+        FLC(fl_dev_tp_unshard_v(P.logits_gather, P.world, 1, P.vocab_stride, P.vocab_first, P.vocab_count, nullptr, P.logits_all));
+    }
 }
 
 // returns true when the graph was executed through the fused plan
@@ -1897,9 +1980,13 @@ bool run_prompt_plan(const ggml_context *ctx, ggml_cgraph *g, void *ev0, void *e
     EvalGraph E;
     if (!parse_eval_graph(g, E) || E.N < 2) return false;
     const int N = E.N, n_embd = E.n_embd, n_ff = E.n_ff, n_vocab = E.n_vocab, hd = E.hd, n_past = E.n_past;
-    if (E.n_head % world != 0 || n_ff % world != 0 || n_vocab % world != 0) return false;
-    const int hl = E.n_head / world, nl = n_embd / world, fl = n_ff / world, vl = n_vocab / world;
-    const size_t slice = ((size_t)N * std::max(nl, std::max(fl, vl)) + 63) & ~(size_t)63;      // floats; keeps recv 256-byte aligned
+    // the decode plan's partition (tp_partition), so both plans read the same shards and the KV cache the same heads; uneven slices
+    // need fl_dev_tp_unshard_v, and a rank that would own nothing sends the eval to the replicated executor
+    const TpPart T = tp_partition(n_embd, hd, n_ff, n_vocab, world);
+    if (!T.ok || (!T.even && (!fl_dev_tp_unshard_v || world > 8))) return false;
+    const int e0 = T.e[rank].first, nl = T.e[rank].rows, f0 = T.f[rank].first, fl = T.f[rank].rows, v0 = T.v[rank].first, vl = T.v[rank].rows;
+    const int h0 = e0 / hd, hl = nl / hd;
+    const size_t slice = ((size_t)N * std::max(T.max_e, std::max(T.max_f, T.max_v)) + 63) & ~(size_t)63;   // floats; keeps recv 256-byte aligned
     if (g_pws.cap < slice) {
         if (g_pws.send) FLC(fl_dev_free(g_pws.send));
         g_pws.send = (float *)fl_dev_malloc(slice * sizeof(float) * (size_t)(world + 1));
@@ -1923,9 +2010,19 @@ bool run_prompt_plan(const ggml_context *ctx, ggml_cgraph *g, void *ev0, void *e
     auto gemm = [&](const ggml_tensor *w, int row0, int rows, const void *q8, float *dst, size_t ldd) {
         mul_mat_q_cols((int)w->type, tp_shard(w, SH_ROWS, row0, rows), w->nb[1], rows, (int)w->ne[0], q8, N, dst, ldd);
     };
-    auto gather = [&](int n_local, const float *residual, float *dst) {
-        FLC(fl_comm_allgather_f32(send, recv, (size_t)N * n_local));
-        FLC(fl_dev_tp_unshard(recv, world, N, n_local, residual, dst));
+    // every rank's [N][rows] slice of one kind of split (T.e, T.f or T.v) -> the eval's [N][n], + residual
+    auto gather = [&](const std::vector<TpSplit> &s, const float *residual, float *dst) {
+        if (T.even) {
+            FLC(fl_comm_allgather_f32(send, recv, (size_t)N * s[0].rows));
+            FLC(fl_dev_tp_unshard(recv, world, N, s[0].rows, residual, dst));
+            return;
+        }
+        // uneven slices: NCCL gathers equal counts, so every rank sends N times the largest slice
+        int first[8], count[8], stride = 0;
+        tp_tables(s, first, count);
+        for (int r = 0; r < world; r++) stride = std::max(stride, count[r]);
+        FLC(fl_comm_allgather_f32(send, recv, (size_t)N * stride));
+        FLC(fl_dev_tp_unshard_v(recv, world, N, stride, first, count, residual, dst));
     };
     auto norm = [&](const ggml_tensor *nrm, const ggml_tensor *rep, const ggml_tensor *mul, const ggml_tensor *gamma) {
         fl_view s = view_of(nrm->src0, ctx), d = view_of(nrm, ctx);
@@ -1945,22 +2042,22 @@ bool run_prompt_plan(const ggml_context *ctx, ggml_cgraph *g, void *ev0, void *e
     for (const LayerNodes &L : E.layers) {
         norm(L.an, L.arep, L.ab, L.attn_norm);
         const void *q8 = q8_of(L.ab);
-        // K, V and Q of this rank's heads: rows [rank * nl, +nl) of wk / wv / wq, written to the same rows of the graph's [N][n_embd] results
-        gemm(L.mk->src0, rank * nl, nl, q8, f32(L.mk) + (size_t)rank * nl, n_embd);
-        fl_view k = sub(view_of(L.rk, ctx), 1, (int64_t)rank * hl, hl);
+        // K, V and Q of this rank's heads: rows [e0, +nl) of wk / wv / wq, written to the same rows of the graph's [N][n_embd] results
+        gemm(L.mk->src0, e0, nl, q8, f32(L.mk) + (size_t)e0, n_embd);
+        fl_view k = sub(view_of(L.rk, ctx), 1, (int64_t)h0, hl);
         FLC(fl_dev_rope(&k, n_past, hd, 0));
         mark_device_write(L.ck->data, ctx);
-        fl_view kslot = dense3((char *)f32(L.vk) + (size_t)rank * nl * 4, hd, hl, N, (int64_t)hd * 4, (int64_t)n_embd * 4);
+        fl_view kslot = dense3((char *)f32(L.vk) + (size_t)e0 * 4, hd, hl, N, (int64_t)hd * 4, (int64_t)n_embd * 4);
         FLC(fl_dev_cpy_f32(&k, &kslot));
-        gemm(L.mv->src0, rank * nl, nl, q8, f32(L.mv) + (size_t)rank * nl, n_embd);
-        fl_view v = sub(view_of(L.tv, ctx), 1, (int64_t)rank * nl, nl), vslot = sub(view_of(L.vv, ctx), 1, (int64_t)rank * nl, nl);
+        gemm(L.mv->src0, e0, nl, q8, f32(L.mv) + (size_t)e0, n_embd);
+        fl_view v = sub(view_of(L.tv, ctx), 1, (int64_t)e0, nl), vslot = sub(view_of(L.vv, ctx), 1, (int64_t)e0, nl);
         mark_device_write(L.cv->data, ctx);
         FLC(fl_dev_cpy_f32(&v, &vslot));
-        gemm(L.mq->src0, rank * nl, nl, q8, f32(L.mq) + (size_t)rank * nl, n_embd);
-        fl_view q = sub(view_of(L.rq, ctx), 1, (int64_t)rank * hl, hl);
+        gemm(L.mq->src0, e0, nl, q8, f32(L.mq) + (size_t)e0, n_embd);
+        fl_view q = sub(view_of(L.rq, ctx), 1, (int64_t)h0, hl);
         FLC(fl_dev_rope(&q, n_past, hd, 0));
         // attention of this rank's heads (axis 2 of every operand)
-        auto heads = [&](const ggml_tensor *t) { return sub(view_of(t, ctx), 2, (int64_t)rank * hl, hl); };
+        auto heads = [&](const ggml_tensor *t) { return sub(view_of(t, ctx), 2, (int64_t)h0, hl); };
         fl_view K = heads(L.Kp), Q = heads(L.pq), S = heads(L.kq), sc = heads(L.sc), mk = heads(L.mask), sm = heads(L.sm), Vh = heads(L.Vv), O = heads(L.kqv);
         FLC(fl_dev_mul_mat_f32(&K, &Q, &S));
         FLC(fl_dev_scale(&sc, E.scale));
@@ -1968,27 +2065,27 @@ bool run_prompt_plan(const ggml_context *ctx, ggml_cgraph *g, void *ev0, void *e
         FLC(fl_dev_soft_max(&sm));
         FLC(fl_dev_mul_mat_f32(&Vh, &sm, &O));
         // this rank's heads of the merged [N][n_embd] attention output -> its [N][nl] slice; gather; wo on this rank's rows
-        fl_view pm = sub(view_of(L.pm, ctx), 1, (int64_t)rank * hl, hl), a = dense3(send, hd, hl, N, (int64_t)hd * 4, (int64_t)nl * 4);
+        fl_view pm = sub(view_of(L.pm, ctx), 1, (int64_t)h0, hl), a = dense3(send, hd, hl, N, (int64_t)hd * 4, (int64_t)nl * 4);
         FLC(fl_dev_cpy_f32(&pm, &a));
-        gather(nl, nullptr, f32(L.att));
-        gemm(L.mo->src0, rank * nl, nl, q8_of(L.att), send, nl);
-        gather(nl, f32(L.ff->src1), f32(L.ff));                                  // + the layer's input
+        gather(T.e, nullptr, f32(L.att));
+        gemm(L.mo->src0, e0, nl, q8_of(L.att), send, nl);
+        gather(T.e, f32(L.ff->src1), f32(L.ff));                                  // + the layer's input
         // feed-forward: w1 / w3 on this rank's n_ff slice, silu * mul of it, gather H, w2 on this rank's rows
         norm(L.cn, L.crep, L.d, L.ffn_norm);
         const void *q8d = q8_of(L.d);
-        gemm(L.m1->src0, rank * fl, fl, q8d, f32(L.m1) + (size_t)rank * fl, n_ff);
-        gemm(L.m3->src0, rank * fl, fl, q8d, f32(L.m3) + (size_t)rank * fl, n_ff);
-        fl_view m1 = sub(view_of(L.m1, ctx), 0, (int64_t)rank * fl, fl), s1 = sub(view_of(L.s1, ctx), 0, (int64_t)rank * fl, fl);
+        gemm(L.m1->src0, f0, fl, q8d, f32(L.m1) + (size_t)f0, n_ff);
+        gemm(L.m3->src0, f0, fl, q8d, f32(L.m3) + (size_t)f0, n_ff);
+        fl_view m1 = sub(view_of(L.m1, ctx), 0, (int64_t)f0, fl), s1 = sub(view_of(L.s1, ctx), 0, (int64_t)f0, fl);
         FLC(fl_dev_silu(&m1, &s1));
-        fl_view m3 = sub(view_of(L.m3, ctx), 0, (int64_t)rank * fl, fl), hs = dense3(send, fl, N, 1, (int64_t)fl * 4, (int64_t)fl * 4 * N);
+        fl_view m3 = sub(view_of(L.m3, ctx), 0, (int64_t)f0, fl), hs = dense3(send, fl, N, 1, (int64_t)fl * 4, (int64_t)fl * 4 * N);
         FLC(fl_dev_mul(&s1, &m3, &hs));
-        gather(fl, nullptr, f32(L.h));
-        gemm(L.m2->src0, rank * nl, nl, q8_of(L.h), send, nl);
-        gather(nl, f32(L.ff), f32(L.xo));                                        // + the attention block's output
+        gather(T.f, nullptr, f32(L.h));
+        gemm(L.m2->src0, e0, nl, q8_of(L.h), send, nl);
+        gather(T.e, f32(L.ff), f32(L.xo));                                        // + the attention block's output
     }
     norm(E.e, E.erep, E.f, E.out_norm);
-    gemm(E.lg->src0, rank * vl, vl, q8_of(E.f), send, vl);
-    gather(vl, nullptr, f32(E.lg));
+    gemm(E.lg->src0, v0, vl, q8_of(E.f), send, vl);
+    gather(T.v, nullptr, f32(E.lg));
     FLC(fl_event_record(ev1));
     // what the caller reads on the host (reference lib/llama.cpp:476-489): the logits of all N columns and the embeddings (the LM head's input)
     FLC(fl_d2h(E.lg->data, f32(E.lg), nbytes_of(E.lg)));
@@ -1996,7 +2093,7 @@ bool run_prompt_plan(const ggml_context *ctx, ggml_cgraph *g, void *ev0, void *e
     FLC(fl_sync());
 
     DecodeState &D = state_for(arena_of(E.layers[0].Kv->data), ctx);
-    D.tp_kv.n_embd = n_embd; D.tp_kv.n_ctx = E.n_ctx;
+    D.tp_kv.n_embd = n_embd; D.tp_kv.n_ctx = E.n_ctx; D.tp_kv.hd = hd;
     D.tp_kv.k.clear(); D.tp_kv.v.clear();
     for (const LayerNodes &L : E.layers) { D.tp_kv.k.push_back(f32(L.Kv)); D.tp_kv.v.push_back(f32(L.Vv)); }
     tp_kv_written(D, n_past, n_past + N);
@@ -2032,32 +2129,39 @@ static void decode_state_release() {
 }
 
 // Tensor-parallel decode steps and prompt-plan evals write only this rank's heads of the new positions into the KV cache (K [pos][n_embd]:
-// nl columns per row; V [n_embd][n_ctx]: nl rows).  Before anything reads the cache as a whole -- save_state, a replicated multi-token
-// eval -- the ranks exchange those slices: pack (strided copies) -> one all-gather -> unpack.  Collective.
+// this rank's columns of every row; V [n_embd][n_ctx]: its rows), the heads tp_partition gives it.  Before anything reads the cache as
+// a whole -- save_state, a replicated multi-token eval -- the ranks exchange those slices: pack (strided copies, each rank's slices
+// padded to the largest one) -> one all-gather -> unpack with every peer's own (first, count).  Collective.
 static void tp_gather_kv(DecodeState &D) {
     const auto &G = D.tp_kv;
     const int world = fl_comm_world(), rank = fl_comm_rank();
     if (!D.tp_kv_sharded || world <= 1 || G.k.empty()) { D.tp_kv_sharded = false; return; }
     const int npos = D.tp_end_pos - D.tp_first_pos, first = D.tp_first_pos;
-    const int n_embd = G.n_embd, n_ctx = G.n_ctx, nl = n_embd / world, L = (int)G.k.size();
-    const size_t per_layer = (size_t)2 * npos * nl, count = per_layer * L;
+    const int n_embd = G.n_embd, n_ctx = G.n_ctx, L = (int)G.k.size();
+    const TpSplit mine = tp_split(n_embd, G.hd, world, rank);
+    int ml = 0;                                                  // the largest slice: every rank's share of the all-gather
+    for (int r = 0; r < world; r++) ml = std::max(ml, tp_split(n_embd, G.hd, world, r).rows);
+    const int nl = mine.rows;
+    const size_t per_layer = (size_t)2 * npos * ml, count = per_layer * L;       // K at [0, npos * nl), V at [npos * ml, +nl * npos)
     float *send = (float *)fl_dev_malloc(count * sizeof(float) * (size_t)(world + 1));
     if (!send) B200_FAIL("KV gather: %s", fl_last_error());
     float *recv = send + count;
     for (int l = 0; l < L; l++) {
-        const float *kmine = G.k[l] + (size_t)first * n_embd + (size_t)rank * nl;          // this rank's columns of K [pos][n_embd]
-        const float *vmine = G.v[l] + (size_t)rank * nl * n_ctx + first;                   // this rank's rows of V [n_embd][n_ctx]
+        const float *kmine = G.k[l] + (size_t)first * n_embd + (size_t)mine.first;        // this rank's columns of K [pos][n_embd]
+        const float *vmine = G.v[l] + (size_t)mine.first * n_ctx + first;                 // this rank's rows of V [n_embd][n_ctx]
         FLC(fl_d2d_2d(send + l * per_layer, (size_t)nl * 4, kmine, (size_t)n_embd * 4, (size_t)nl * 4, (size_t)npos));
-        FLC(fl_d2d_2d(send + l * per_layer + (size_t)npos * nl, (size_t)npos * 4, vmine, (size_t)n_ctx * 4, (size_t)npos * 4, (size_t)nl));
+        FLC(fl_d2d_2d(send + l * per_layer + (size_t)npos * ml, (size_t)npos * 4, vmine, (size_t)n_ctx * 4, (size_t)npos * 4, (size_t)nl));
     }
     FLC(fl_comm_allgather_f32(send, recv, count));
     for (int r = 0; r < world; r++) {
         if (r == rank) continue;
+        const TpSplit peer = tp_split(n_embd, G.hd, world, r);
+        const size_t pl = (size_t)peer.rows;
         for (int l = 0; l < L; l++) {
             float *kbase = G.k[l], *vbase = G.v[l];
             const float *src = recv + (size_t)r * count + l * per_layer;
-            FLC(fl_d2d_2d(kbase + (size_t)first * n_embd + (size_t)r * nl, (size_t)n_embd * 4, src, (size_t)nl * 4, (size_t)nl * 4, (size_t)npos));
-            FLC(fl_d2d_2d(vbase + (size_t)r * nl * n_ctx + first, (size_t)n_ctx * 4, src + (size_t)npos * nl, (size_t)npos * 4, (size_t)npos * 4, (size_t)nl));
+            FLC(fl_d2d_2d(kbase + (size_t)first * n_embd + (size_t)peer.first, (size_t)n_embd * 4, src, pl * 4, pl * 4, (size_t)npos));
+            FLC(fl_d2d_2d(vbase + (size_t)peer.first * n_ctx + first, (size_t)n_ctx * 4, src + (size_t)npos * ml, (size_t)npos * 4, (size_t)npos * 4, pl));
         }
     }
     FLC(fl_sync());
@@ -2164,9 +2268,9 @@ extern "C" void ggml_graph_compute(struct ggml_context *ctx, struct ggml_cgraph 
         mark_device_write(dout.kv_host, ctx);          // the step appended one position to the KV cache on the device
         if (fl_comm_world() > 1) {
             const DecodePlan &P = D.plan;
-            const size_t own = (size_t)fl_comm_rank() * (size_t)(P.n_embd / P.world);     // the plan's cache pointers are offset to this rank's heads
+            const size_t own = (size_t)P.embd_first;              // the plan's cache pointers are offset to this rank's heads
             auto &G = D.tp_kv;
-            G.n_embd = P.n_embd; G.n_ctx = P.n_ctx;
+            G.n_embd = P.n_embd; G.n_ctx = P.n_ctx; G.hd = P.n_embd / P.n_head;
             G.k.clear(); G.v.clear();
             for (const LayerPlan &L : P.layers) { G.k.push_back((float *)L.kcache - own); G.v.push_back((float *)L.vcache - own * P.n_ctx); }
             const int pos = S.h_scalars[0];                       // n_past of this step = the position it wrote

@@ -135,6 +135,8 @@ SIGNATURES = {
 LAZY_SIGNATURES = {
     "fl_dev_quantize_q4_file": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "fl_dev_tp_unshard": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "fl_dev_tp_unshard_v": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p,
+                                      C.c_void_p]),
     "fl_dev_add_q_f16": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]),
     "fl_dev_scale_f16": (C.c_int, [_VP, C.c_float]),
 }

@@ -174,6 +174,12 @@ int fl_dev_mul_mat_f32(const fl_view *src0, const fl_view *src1, const fl_view *
  * every row).  residual (nullable, [N][world * n_local]) is added with one fp32 rounding per element -- the bits of ggml_add --
  * so the gather after wo / w2 needs no separate add.  dst must not overlap `gathered`; it may be `residual`. */
 int fl_dev_tp_unshard(const float *gathered, int world, int N, int n_local, const float *residual, float *dst);
+/* The same for uneven slices (world 1..8): rank r's [N][count[r]] block sits at gathered + r * N * slice_stride (an all-gather of
+ * slices padded to slice_stride floats) and goes to columns [first[r], first[r] + count[r]) of [N][n], n = sum of count[].  first[]
+ * and count[] are host arrays of `world` entries; the slices must tile [0, n).  float4 accesses for the ranks whose slice allows
+ * them, scalar ones for the others; residual and the overlap rules as above. */
+int fl_dev_tp_unshard_v(const float *gathered, int world, int N, int slice_stride, const int *first, const int *count, const float *residual,
+                        float *dst);
 
 /* ---- fused decode step (N = 1) ------------------------------------------------------------------
  * fl_dev_mv_fused: up to three weight matrices that share one input, one launch.  The prologue builds
