@@ -139,6 +139,59 @@ def write_synthetic_float(path, ftype=F16, n_vocab=512, n_embd=256, n_mult=64, n
                             vocab_entries(n_vocab), tensors())
 
 
+def splits_by_columns(name: str) -> bool:
+    """The tensors the reference's reader joins from column ranges when a model comes in parts (the token embeddings,
+    wo and w2: include/tensor/utils.hpp:101-106); every other matrix is joined from row ranges."""
+    return name.startswith("tok_embeddings.") or name.endswith((".attention.wo.weight", ".feed_forward.w2.weight"))
+
+
+def _shard(name, idx, ne, ftype, n_parts, j, seed, std):
+    """Part j's shard of tensor idx (tensor_plan order) of a split synthetic model: (shard ne, type, bytes).  Each
+    shard is its own Gaussian stream; vectors are ones, whole in every part."""
+    if len(ne) == 1:
+        return ne, F32, np.ones(ne[0], dtype=np.float32).tobytes()
+    k, m = ne
+    shape = (m, k // n_parts) if splits_by_columns(name) else (m // n_parts, k)
+    w = np.random.default_rng([seed, idx, j]).standard_normal(shape, dtype=np.float32)
+    w *= np.float32(1.0 if name.startswith("tok_embeddings") else std)
+    return (shape[1], shape[0]), ftype, w.astype(FLOAT_DTYPE[ftype], copy=False).tobytes()
+
+
+def write_synthetic_parts(base, fmts, ftype=F16, n_vocab=512, n_embd=256, n_mult=64, n_head=4, n_layer=2, seed=0, std=0.02,
+                          edit=None) -> str:
+    """An unquantised model split into len(fmts) parts the way the reference's converter writes one per checkpoint
+    shard: part j, in format fmts[j], goes to base (j = 0) or base.j, every part with the full model's header and
+    vocab.  edit(j, hparams, tensors) -> (hparams, tensors) changes a part before it is written (tests).  Shards are
+    generated one at a time unless edit needs a part's list."""
+    hp = (n_vocab, n_embd, n_mult, n_head, n_layer, n_embd // n_head, ftype)
+    plan = list(tensor_plan(n_vocab, n_embd, n_mult, n_head, n_layer))
+    for j, fmt in enumerate(fmts):
+        tensors = ((name, *_shard(name, i, ne, ftype, len(fmts), j, seed, std)) for i, (name, ne) in enumerate(plan))
+        hp_j = hp
+        if edit is not None:
+            hp_j, tensors = edit(j, hp, list(tensors))
+        write_model_file(base if j == 0 else f"{base}.{j}", fmt, hp_j, vocab_entries(n_vocab), tensors)
+    return base
+
+
+def write_synthetic_joined(path, n_parts, ftype=F16, n_vocab=512, n_embd=256, n_mult=64, n_head=4, n_layer=2, seed=0,
+                           std=0.02, fmt="ggjt") -> str:
+    """The model write_synthetic_parts splits into n_parts parts, as one file: every matrix its shards joined by
+    columns or by rows (splits_by_columns), every vector part 0's."""
+    def tensors():
+        for i, (name, ne) in enumerate(tensor_plan(n_vocab, n_embd, n_mult, n_head, n_layer)):
+            shards = [_shard(name, i, ne, ftype, n_parts, j, seed, std) for j in range(n_parts)]
+            if len(ne) == 1:
+                yield name, ne, F32, shards[0][2]
+                continue
+            arrs = [np.frombuffer(b, dtype=FLOAT_DTYPE[ftype]).reshape(sne[1], sne[0]) for sne, _, b in shards]
+            yield name, ne, ftype, np.concatenate(arrs, axis=1 if splits_by_columns(name) else 0).tobytes()
+
+    write_model_file(path, fmt, (n_vocab, n_embd, n_mult, n_head, n_layer, n_embd // n_head, ftype), vocab_entries(n_vocab),
+                     tensors())
+    return path
+
+
 def write_synthetic_numpy(path, wtype=Q4_0, n_vocab=512, n_embd=256, n_mult=64, n_head=4, n_layer=2, seed=0, std=0.02,
                           quantize=None) -> int:
     """CPU generator for toy models (tests).  `quantize(w_f32[M,K], wtype) -> uint8` must follow the
