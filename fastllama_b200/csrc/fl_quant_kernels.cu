@@ -66,12 +66,20 @@ __device__ __forceinline__ int fl_quantize_block_q4_0(float v, int lane, fl_bloc
     return q & 0xF;
 }
 
+// FIRST_MIN: m is the block's first element equal to the minimum, as the reference's `if (v < min)`
+// scan keeps it.  That differs from the fminf tree only in the sign of a zero minimum, when the block
+// holds both +0 and -0 (as f32 values below 2^-25 do once rounded to f16).
+template <bool FIRST_MIN = false>
 __device__ __forceinline__ int fl_quantize_block_q4_1(float v, int lane, fl_block_q4_1 *yb) {
     float mn = v, mx = v;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
         mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    }
+    if (FIRST_MIN) {
+        const unsigned at = __ballot_sync(0xffffffffu, v == mn);
+        if (at) mn = __shfl_sync(0xffffffffu, v, __ffs(at) - 1);
     }
     const float d = __fdiv_rn(__fsub_rn(mx, mn), 15.0f);
     const float id = (d != 0.0f) ? __fdiv_rn(1.0f, d) : 0.0f;
@@ -102,11 +110,15 @@ __global__ void k_quantize_q4_1(const float *__restrict__ x, fl_block_q4_1 *__re
 // Model-file quantisation (the reference's fastllama::quantize, lib/llama.cpp:585-646): a tensor's
 // rows as the input file stores them, f32 or f16, to q4 blocks, plus the 16-bin histogram of the
 // stored nibbles that ggml_quantize_chunk reports.  f16 -> f32 is exact, so __half2float gives the
-// reference's ggml_fp16_to_fp32 inputs and the blocks carry the bits of k_quantize_q4_*.
+// reference's ggml_fp16_to_fp32 inputs and the blocks carry the bits of k_quantize_q4_*, except that a
+// q4_1 block's m keeps the sign of its first zero when its minimum is a zero of both signs.  SRC 2 is
+// f32 rounded to f16 (round to nearest even, as numpy's astype(float16) in the reference's converter)
+// and widened back: the values the reference's tool reads from the f16 file converted from an f32
+// checkpoint.
 // Histogram: four ballots (one per bit of the nibble) give every lane the warp's count for bin
 // `lane` (lanes 0..15); the counts stay in a register across the warp's blocks, then go through
 // shared memory to one set of 16 64-bit global atomics per CTA.
-template <int TYPE, bool F16>
+template <int TYPE, int SRC>
 __global__ void __launch_bounds__(256) k_quantize_q4_file(const void *__restrict__ x, void *__restrict__ y, long nblocks,
                                                           unsigned long long *__restrict__ hist) {
     __shared__ unsigned sh_hist[16];
@@ -117,9 +129,11 @@ __global__ void __launch_bounds__(256) k_quantize_q4_file(const void *__restrict
     const long nw = ((long)gridDim.x * blockDim.x) >> 5;
     unsigned cnt = 0;                                        // lanes 0..15: this warp's count of nibble value `lane`
     for (long b = wid; b < nblocks; b += nw) {
-        const float v = F16 ? __half2float(((const __half *)x)[b * FL_QK + lane]) : ((const float *)x)[b * FL_QK + lane];
+        const float v = SRC == 1   ? __half2float(((const __half *)x)[b * FL_QK + lane])
+                        : SRC == 2 ? __half2float(__float2half_rn(((const float *)x)[b * FL_QK + lane]))
+                                   : ((const float *)x)[b * FL_QK + lane];
         const int q = (TYPE == FL_TYPE_Q4_0) ? fl_quantize_block_q4_0(v, lane, (fl_block_q4_0 *)y + b)
-                                             : fl_quantize_block_q4_1(v, lane, (fl_block_q4_1 *)y + b);
+                                             : fl_quantize_block_q4_1<true>(v, lane, (fl_block_q4_1 *)y + b);
         unsigned m = 0xffffffffu;
 #pragma unroll
         for (int j = 0; j < 4; j++) {
@@ -482,20 +496,23 @@ int flk_quantize_q4(cudaStream_t st, int type, const float *x, void *y, int k, i
     return 0;
 }
 
-int flk_quantize_q4_file(cudaStream_t st, int type, int src_f16, const void *x, void *y, int k, int nrows,
+int flk_quantize_q4_file(cudaStream_t st, int type, int src_type, const void *x, void *y, int k, int nrows,
                          unsigned long long *hist) {
     FL_REQUIRE(k > 0 && k % FL_QK == 0, "quantize_q4_file: k=%d is not a multiple of 32", k);
     FL_REQUIRE(type == FL_TYPE_Q4_0 || type == FL_TYPE_Q4_1, "quantize_q4_file: unsupported type %d (q4_0 = 2, q4_1 = 3)", type);
-    FL_REQUIRE(src_f16 == 0 || src_f16 == 1, "quantize_q4_file: unsupported source type %d (0 f32, 1 f16)", src_f16);
+    FL_REQUIRE(src_type >= 0 && src_type <= 2, "quantize_q4_file: unsupported source type %d (0 f32, 1 f16, 2 f32 via f16)",
+               src_type);
     if (nrows <= 0) return 0;
     const long nblocks = (long)(k / FL_QK) * nrows;
     const int grid = grid_for_warps(nblocks, 256);
     if (type == FL_TYPE_Q4_0) {
-        if (src_f16) k_quantize_q4_file<FL_TYPE_Q4_0, true><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
-        else k_quantize_q4_file<FL_TYPE_Q4_0, false><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
+        if (src_type == 1) k_quantize_q4_file<FL_TYPE_Q4_0, 1><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
+        else if (src_type == 2) k_quantize_q4_file<FL_TYPE_Q4_0, 2><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
+        else k_quantize_q4_file<FL_TYPE_Q4_0, 0><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
     } else {
-        if (src_f16) k_quantize_q4_file<FL_TYPE_Q4_1, true><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
-        else k_quantize_q4_file<FL_TYPE_Q4_1, false><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
+        if (src_type == 1) k_quantize_q4_file<FL_TYPE_Q4_1, 1><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
+        else if (src_type == 2) k_quantize_q4_file<FL_TYPE_Q4_1, 2><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
+        else k_quantize_q4_file<FL_TYPE_Q4_1, 0><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
     }
     fl_count_launch();
     FL_CUDA_OK(cudaGetLastError());

@@ -133,6 +133,7 @@ SIGNATURES = {
 # Bound on first use (FlCuda.fn) rather than at load, so that a stand-in library without them still loads for
 # everything else.  libfl_cuda.so exports them like every function of include/fl_cuda.h.
 LAZY_SIGNATURES = {
+    # type, src_type (0 f32, 1 f16, 2 f32 rounded to f16 and widened back), x, y, k, nrows, hist
     "fl_dev_quantize_q4_file": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "fl_dev_tp_unshard": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "fl_dev_tp_unshard_v": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p,

@@ -112,7 +112,9 @@ int fl_dev_quantize_q4(int type, const float *x, void *y, int k, int nrows);
 
 /* Model-file quantisation (the tensor loop of fastllama::quantize, lib/llama.cpp:585-646): nrows rows
  * of k elements as the input file stores them (src_type 0 = f32, 1 = f16; f16 converts exactly like
- * ggml_fp16_to_fp32) -> q4_0 / q4_1 blocks with the bits of fl_quantize_rows_q4.  hist_dev (16
+ * ggml_fp16_to_fp32; 2 = f32 rounded to f16, nearest even, and widened back, the values of an f32
+ * checkpoint after the reference converter's f16 step) -> q4_0 / q4_1 blocks with the bits of
+ * fl_quantize_rows_q4.  hist_dev (16
  * counters, may be NULL) is incremented by the count of each stored nibble value, the histogram
  * ggml_quantize_chunk reports.  Asynchronous on the library stream, like every fl_dev_* call. */
 int fl_dev_quantize_q4_file(int type, int src_type, const void *x_dev, void *y_dev, int k, int nrows,
