@@ -18,6 +18,8 @@ int flk_quantize_q8_0(cudaStream_t st, const float *x, size_t x_row_stride_bytes
 int flk_quantize_q4(cudaStream_t st, int type, const float *x, void *y, int k, int nrows);
 int flk_quantize_q4_file(cudaStream_t st, int type, int src_type, const void *x, void *y, int k, int nrows,
                          unsigned long long *hist);
+int flk_quantize_q4_file_lora(cudaStream_t st, int type, int src_type, const void *x, int delta_type, const void *delta, void *y, int k,
+                              int nrows, unsigned long long *hist);
 int flk_dequantize_rows(cudaStream_t st, int type, const void *W, size_t w_row_stride, int K, const int32_t *ids,
                         int n_ids, float *dst, size_t dst_row_stride);
 int flk_mul_mat_q(cudaStream_t st, int type, const void *W, size_t w_row_stride, int M, int K, const void *Yq8, int N,

@@ -114,13 +114,22 @@ __global__ void k_quantize_q4_1(const float *__restrict__ x, fl_block_q4_1 *__re
 // q4_1 block's m keeps the sign of its first zero when its minimum is a zero of both signs.  SRC 2 is
 // f32 rounded to f16 (round to nearest even, as numpy's astype(float16) in the reference's converter)
 // and widened back: the values the reference's tool reads from the f16 file converted from an f32
-// checkpoint.
+// checkpoint.  SRC 3 is f16 data of an f32 file (an f16 checkpoint converted to f32): the values of
+// SRC 1, merged by the f32 rule below.
+// DELTA (FL_DELTA_F32 / FL_DELTA_F16): a LoRA delta of the same [rows][k] layout is merged first, as
+// the reference's attach_lora merges it into an unquantised model (ggml_add_inplace, lib/ggml.c):
+// into an f32 file (SRC 0, 3) w + d (add_f32); into an f16 file (SRC 1, 2; for SRC 2 w is already the
+// f16-rounded value) fp16_rn(w + fp32(d)) (add_f16_f32 / add_f16_f16: widening f16 is exact, so both
+// are this one formula), then widened back for the quantiser.
 // Histogram: four ballots (one per bit of the nibble) give every lane the warp's count for bin
 // `lane` (lanes 0..15); the counts stay in a register across the warp's blocks, then go through
 // shared memory to one set of 16 64-bit global atomics per CTA.
-template <int TYPE, int SRC>
-__global__ void __launch_bounds__(256) k_quantize_q4_file(const void *__restrict__ x, void *__restrict__ y, long nblocks,
-                                                          unsigned long long *__restrict__ hist) {
+#define FL_DELTA_NONE (-1)
+#define FL_DELTA_F32 0
+#define FL_DELTA_F16 1
+template <int TYPE, int SRC, int DELTA>
+__global__ void __launch_bounds__(256) k_quantize_q4_file(const void *__restrict__ x, const void *__restrict__ delta, void *__restrict__ y,
+                                                          long nblocks, unsigned long long *__restrict__ hist) {
     __shared__ unsigned sh_hist[16];
     const int lane = threadIdx.x & 31;
     if (threadIdx.x < 16) sh_hist[threadIdx.x] = 0;
@@ -129,9 +138,15 @@ __global__ void __launch_bounds__(256) k_quantize_q4_file(const void *__restrict
     const long nw = ((long)gridDim.x * blockDim.x) >> 5;
     unsigned cnt = 0;                                        // lanes 0..15: this warp's count of nibble value `lane`
     for (long b = wid; b < nblocks; b += nw) {
-        const float v = SRC == 1   ? __half2float(((const __half *)x)[b * FL_QK + lane])
-                        : SRC == 2 ? __half2float(__float2half_rn(((const float *)x)[b * FL_QK + lane]))
-                                   : ((const float *)x)[b * FL_QK + lane];
+        const long e = b * FL_QK + lane;
+        float v = (SRC == 1 || SRC == 3) ? __half2float(((const __half *)x)[e])
+                  : SRC == 2             ? __half2float(__float2half_rn(((const float *)x)[e]))
+                                         : ((const float *)x)[e];
+        if (DELTA != FL_DELTA_NONE) {
+            const float d = DELTA == FL_DELTA_F16 ? __half2float(((const __half *)delta)[e]) : ((const float *)delta)[e];
+            v = __fadd_rn(v, d);
+            if (SRC == 1 || SRC == 2) v = __half2float(__float2half_rn(v));
+        }
         const int q = (TYPE == FL_TYPE_Q4_0) ? fl_quantize_block_q4_0(v, lane, (fl_block_q4_0 *)y + b)
                                              : fl_quantize_block_q4_1<true>(v, lane, (fl_block_q4_1 *)y + b);
         unsigned m = 0xffffffffu;
@@ -496,27 +511,58 @@ int flk_quantize_q4(cudaStream_t st, int type, const float *x, void *y, int k, i
     return 0;
 }
 
-int flk_quantize_q4_file(cudaStream_t st, int type, int src_type, const void *x, void *y, int k, int nrows,
-                         unsigned long long *hist) {
+typedef void (*q4_file_kernel_t)(const void *, const void *, void *, long, unsigned long long *);
+template <int TYPE>
+static q4_file_kernel_t q4_file_kernel(int src_type, int delta_type) {
+    if (delta_type == FL_DELTA_NONE) {
+        switch (src_type) {
+            case 0: return k_quantize_q4_file<TYPE, 0, FL_DELTA_NONE>;
+            case 1: case 3: return k_quantize_q4_file<TYPE, 1, FL_DELTA_NONE>;      // the same values with nothing to merge
+            case 2: return k_quantize_q4_file<TYPE, 2, FL_DELTA_NONE>;
+        }
+    } else if (delta_type == FL_DELTA_F32) {
+        switch (src_type) {
+            case 0: return k_quantize_q4_file<TYPE, 0, FL_DELTA_F32>;
+            case 1: return k_quantize_q4_file<TYPE, 1, FL_DELTA_F32>;
+            case 2: return k_quantize_q4_file<TYPE, 2, FL_DELTA_F32>;
+            case 3: return k_quantize_q4_file<TYPE, 3, FL_DELTA_F32>;
+        }
+    } else if (delta_type == FL_DELTA_F16) {
+        switch (src_type) {
+            case 1: return k_quantize_q4_file<TYPE, 1, FL_DELTA_F16>;
+            case 2: return k_quantize_q4_file<TYPE, 2, FL_DELTA_F16>;
+        }
+    }
+    return nullptr;
+}
+
+int flk_quantize_q4_file_lora(cudaStream_t st, int type, int src_type, const void *x, int delta_type, const void *delta, void *y, int k,
+                              int nrows, unsigned long long *hist) {
     FL_REQUIRE(k > 0 && k % FL_QK == 0, "quantize_q4_file: k=%d is not a multiple of 32", k);
     FL_REQUIRE(type == FL_TYPE_Q4_0 || type == FL_TYPE_Q4_1, "quantize_q4_file: unsupported type %d (q4_0 = 2, q4_1 = 3)", type);
-    FL_REQUIRE(src_type >= 0 && src_type <= 2, "quantize_q4_file: unsupported source type %d (0 f32, 1 f16, 2 f32 via f16)",
-               src_type);
+    FL_REQUIRE(src_type >= 0 && src_type <= 3,
+               "quantize_q4_file: unsupported source type %d (0 f32, 1 f16, 2 f32 via f16, 3 f16 of an f32 file)", src_type);
+    FL_REQUIRE(delta_type >= FL_DELTA_NONE && delta_type <= FL_DELTA_F16, "quantize_q4_file: unsupported delta type %d (-1 none, 0 f32, 1 f16)",
+               delta_type);
+    FL_REQUIRE((delta_type == FL_DELTA_NONE) == (delta == nullptr), "quantize_q4_file: delta type %d with a %s delta buffer", delta_type,
+               delta ? "non-null" : "null");
+    FL_REQUIRE(!(delta_type == FL_DELTA_F16 && (src_type == 0 || src_type == 3)),
+               "quantize_q4_file: an f16 delta cannot be merged into an f32 file (the reference's add_f32 has no f16 operand)");
     if (nrows <= 0) return 0;
     const long nblocks = (long)(k / FL_QK) * nrows;
-    const int grid = grid_for_warps(nblocks, 256);
-    if (type == FL_TYPE_Q4_0) {
-        if (src_type == 1) k_quantize_q4_file<FL_TYPE_Q4_0, 1><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
-        else if (src_type == 2) k_quantize_q4_file<FL_TYPE_Q4_0, 2><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
-        else k_quantize_q4_file<FL_TYPE_Q4_0, 0><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
-    } else {
-        if (src_type == 1) k_quantize_q4_file<FL_TYPE_Q4_1, 1><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
-        else if (src_type == 2) k_quantize_q4_file<FL_TYPE_Q4_1, 2><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
-        else k_quantize_q4_file<FL_TYPE_Q4_1, 0><<<grid, 256, 0, st>>>(x, y, nblocks, hist);
-    }
+    const q4_file_kernel_t kern = type == FL_TYPE_Q4_0 ? q4_file_kernel<FL_TYPE_Q4_0>(src_type, delta_type)
+                                                       : q4_file_kernel<FL_TYPE_Q4_1>(src_type, delta_type);
+    kern<<<grid_for_warps(nblocks, 256), 256, 0, st>>>(x, delta, y, nblocks, hist);
     fl_count_launch();
     FL_CUDA_OK(cudaGetLastError());
     return 0;
+}
+
+int flk_quantize_q4_file(cudaStream_t st, int type, int src_type, const void *x, void *y, int k, int nrows,
+                         unsigned long long *hist) {
+    FL_REQUIRE(src_type >= 0 && src_type <= 2, "quantize_q4_file: unsupported source type %d (0 f32, 1 f16, 2 f32 via f16)",
+               src_type);
+    return flk_quantize_q4_file_lora(st, type, src_type, x, FL_DELTA_NONE, nullptr, y, k, nrows, hist);
 }
 
 int flk_dequantize_rows(cudaStream_t st, int type, const void *W, size_t w_row_stride, int K, const int32_t *ids,

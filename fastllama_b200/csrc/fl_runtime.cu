@@ -303,6 +303,12 @@ extern "C" int fl_dev_quantize_q4_file(int type, int src_type, const void *x, vo
     FL_REQUIRE(x && y, "fl_dev_quantize_q4_file: null buffer");
     return flk_quantize_q4_file(g.stream, type, src_type, x, y, k, nrows, hist);
 }
+extern "C" int fl_dev_quantize_q4_file_lora(int type, int src_type, const void *x, int delta_type, const void *delta, void *y, int k, int nrows,
+                                            unsigned long long *hist) {
+    FL_NEED_INIT();
+    FL_REQUIRE(x && y, "fl_dev_quantize_q4_file_lora: null buffer");
+    return flk_quantize_q4_file_lora(g.stream, type, src_type, x, delta_type, delta, y, k, nrows, hist);
+}
 
 extern "C" int fl_dev_quantize_q4_simd(int type, const float *x, void *y, int k, int nrows) {
     FL_NEED_INIT();

@@ -135,6 +135,9 @@ SIGNATURES = {
 LAZY_SIGNATURES = {
     # type, src_type (0 f32, 1 f16, 2 f32 rounded to f16 and widened back), x, y, k, nrows, hist
     "fl_dev_quantize_q4_file": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    # type, src_type (also 3: f16 data of an f32 file), x, delta_type (-1 none, 0 f32, 1 f16), delta, y, k, nrows, hist
+    "fl_dev_quantize_q4_file_lora": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                              C.c_void_p]),
     "fl_dev_tp_unshard": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "fl_dev_tp_unshard_v": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p,
                                       C.c_void_p]),

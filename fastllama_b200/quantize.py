@@ -26,6 +26,13 @@ Input may also be a PyTorch (torch.save zip) or safetensors checkpoint, Meta or 
 directory or its first file: it is quantised as the f16 (outtype "f16", the default) or f32 file the reference's
 scripts/convert.py writes from it (read_checkpoint), in one pass and without writing that file.
 
+With an adapter (lora=, --lora: a file the reference's scripts/convert-lora-to-ggml.py writes, read_lora), the output
+is the reference tool's file for the f16 / f32 model after the reference's attach_lora has merged the adapter into
+it (lib/llama.cpp:697-944): each targeted tensor, as the f16 / f32 file holds it, gets ggml_add_inplace(W, delta)
+with delta the cached `.lora` tensor or mul_mat(loraA, loraB), and is then quantised.  The merge runs inside the
+quantiser's kernel (fl_dev_quantize_q4_file_lora), before the q4 rounding, so none of the adapter is lost to a
+dequantise / requantise round trip, and the merged file needs no attach at load.
+
 Streaming: each part is memory-mapped once and read one shard at a time through two pinned staging chunks, so a
 read from a file overlaps the previous chunk's host-to-device copy, and a tensor's file reads overlap the previous
 tensor's kernel and device-to-host copy; the previous tensor is written to the output while this one's copies run.
@@ -628,15 +635,124 @@ def _src_type(t: Tensor) -> int:
     return t.type if t.src_type < 0 else t.src_type
 
 
+# ------------------------------------------------------------------------------------------------------------ LoRA
+class LoraDelta(NamedTuple):
+    """What one model tensor gets from an adapter: a cached delta (`lora`, [M][K] of `type`) or the f32 pair
+    loraA ([K][rank], already scaled) and loraB ([M][rank]), whose mul_mat is the delta."""
+    base: str
+    type: int              # F32 / F16 of the delta as merged (a loraA / loraB pair: F32)
+    lora: Shard | None
+    a: Shard | None
+    b: Shard | None
+    rank: int              # uncached: the contraction length; cached: 0
+
+
+class LoraAdapter(NamedTuple):
+    path: str
+    cached: bool
+    r: int
+    alpha: int
+    deltas: list           # LoraDelta in the order the reference merges them (the second tensor of a pair completes it)
+
+
+def read_lora(path: str, model: ModelFile) -> LoraAdapter:
+    """Parse the GGLA adapter at path with the reference loader's rules (include/file_loader.hpp: magic 'ggla',
+    version 1, u8 cache flag, u32 r, u32 alpha; per tensor the GGJT entry with data 32-byte aligned) and match it to
+    model as the reference's attach does (lib/llama.cpp:760-910): a cached adapter names `<base>.lora`, an uncached
+    one `<base>.loraA` and `<base>.loraB`.  Refuses, naming the file and the tensor, everything the reference refuses
+    or would merge into garbage, and every tensor the merge would leave unused."""
+    size = os.path.getsize(path)
+    with open(path, "rb") as f:
+        magic, version = struct.unpack("<II", _read(f, 8))
+        if magic != GGLA_MAGIC:
+            raise QuantizeError(f"{path}: bad magic {magic:08x} (not a ggla LoRA adapter)")
+        if version != 1:
+            raise QuantizeError(f"{path}: unsupported adapter version {version} (expected 1)")
+        cached, r, alpha = struct.unpack("<?II", _read(f, 9))
+        entries = {}
+        while f.tell() < size:
+            n_dims, name_len, t = struct.unpack("<III", _read(f, 12))
+            if n_dims < 1 or n_dims > 2:
+                raise QuantizeError(f"{path}: a tensor has {n_dims} dimensions (1 or 2 expected)")
+            ne = struct.unpack(f"<{n_dims}I", _read(f, 4 * n_dims))
+            name = _read(f, name_len).decode("utf-8", errors="replace")
+            if n_dims != 2:
+                raise QuantizeError(f"{path}: tensor '{name}' is {n_dims}-D; the reference's adapter loader takes matrices only")
+            if t not in (F32, F16):
+                what = TYPE_NAMES[t] if t < len(TYPE_NAMES) else f"type {t}"
+                raise QuantizeError(f"{path}: tensor '{name}' is {what}; adapter tensors are f32 or f16")
+            if name in entries:
+                raise QuantizeError(f"{path}: tensor '{name}' appears twice")
+            f.seek(-f.tell() & 31, os.SEEK_CUR)
+            nbytes = ne[0] * ne[1] * ELEM_BYTES[t]
+            off = f.tell()
+            if off + nbytes > size:
+                raise QuantizeError(f"{path}: tensor '{name}' extends past the end of the file")
+            entries[name] = (ne, t, Shard(0, off, nbytes))
+            f.seek(nbytes, os.SEEK_CUR)
+
+    by_name = {t.name: t for t in model.tensors}
+    deltas, pending = [], {}                                # pending: base -> {"A" / "B": (name, ne, t, shard)}
+    for name, (ne, t, sh) in entries.items():
+        suffix = ".lora" if cached else name[-6:] if name[-6:] in (".loraA", ".loraB") else None
+        if suffix is None or not name.endswith(suffix) or len(name) == len(suffix):
+            want = "<base>.lora (a cached adapter)" if cached else "<base>.loraA or <base>.loraB (an uncached adapter)"
+            raise QuantizeError(f"{path}: tensor '{name}' is not a LoRA tensor: expected {want}")
+        base = name[:-len(suffix)]
+        w = by_name.get(base)
+        where = f"{path}: tensor '{name}'"
+        if w is None:
+            raise QuantizeError(f"{where}: its base '{base}' is not a tensor of {model.paths[0]} (unknown tensor in lora adapter)")
+        if len(w.ne) != 2:
+            raise QuantizeError(f"{where}: its base '{base}' is 1-D; only matrices take an adapter here")
+        if not cached and t != F32:
+            raise QuantizeError(f"{where} is f16 in an uncached adapter; the reference merges uncached adapters from f32 "
+                                "tensors only")
+        if cached:
+            if ne != w.ne:
+                raise QuantizeError(f"{where} has extents {ne}, but '{base}' has {w.ne} (incompatible tensor dimensions)")
+            if t == F16 and w.type == F32:
+                raise QuantizeError(f"{where} is f16 and '{base}' is f32: the reference's add_f32 reads an f16 delta as "
+                                    "f32 (use an f32 adapter with an f32 model)")
+            deltas.append(LoraDelta(base, t, sh, None, None, 0))
+            continue
+        half = pending.setdefault(base, {})
+        half[suffix[-1]] = (name, ne, sh)
+        if len(half) < 2:
+            continue
+        (na, a_ne, a_sh), (nb, b_ne, b_sh) = half.pop("A"), half.pop("B")
+        del pending[base]
+        if a_ne[1] != w.ne[0] or b_ne[1] != w.ne[1]:
+            raise QuantizeError(f"{path}: tensors '{na}' {a_ne} and '{nb}' {b_ne} do not give the extents {w.ne} of '{base}' "
+                                "(incompatible tensor dimensions)")
+        if a_ne[0] != b_ne[0]:
+            raise QuantizeError(f"{path}: tensors '{na}' and '{nb}' have ranks {a_ne[0]} and {b_ne[0]}; mul_mat(loraA, loraB) "
+                                "needs one")
+        deltas.append(LoraDelta(base, F32, None, a_sh, b_sh, a_ne[0]))
+    for base, half in pending.items():
+        (name, *_), = half.values()
+        other = name[:-1] + ("B" if name.endswith("A") else "A")
+        raise QuantizeError(f"{path}: tensor '{name}' has no '{other}' (an unpaired LoRA tensor)")
+    return LoraAdapter(path, cached, r, alpha, deltas)
+
+
+def _merge_src(t: Tensor) -> int:
+    """src_type of fl_dev_quantize_q4_file(_lora) for t: its staged type, 2 for an f32 checkpoint's values as the
+    converter's f16 file holds them, 3 for an f16 checkpoint's values in the converter's f32 file (merged in f32)."""
+    return {(F32, F16): 2, (F16, F32): 3}.get((_src_type(t), t.type), _src_type(t))
+
+
 def quantize_model(in_path: str, out_path: str, wtype: int, fl: FlCuda | None = None, verbose: bool = True, *,
-                   outtype: str | None = None, vocab_dir: str | None = None) -> dict:
+                   outtype: str | None = None, vocab_dir: str | None = None, lora: str | None = None) -> dict:
     """Quantise in_path to out_path (q4_0 for wtype 2, q4_1 for 3).  in_path is an f32 / f16 model file (for a model
     in parts, part 0's path) or a PyTorch / safetensors checkpoint (a directory or its first file, see
     read_checkpoint).  A checkpoint is quantised as the f16 (outtype None or "f16") or f32 ("f32") file the reference's
     converter writes from it; vocab_dir is where its tokenizer.model is, if not beside the checkpoint or in its parent.
     outtype and vocab_dir are refused for model files, which carry their types and vocab.  Returns the number of parts
     read, per-tensor and total sizes and the 16-bin histograms of the stored nibbles (counts), as the reference's tool
-    reports them (sizes and types of a checkpoint's tensors are those of the converter's file)."""
+    reports them (sizes and types of a checkpoint's tensors are those of the converter's file).  lora is a LoRA
+    adapter to merge into the f16 / f32 weights before they are quantised (read_lora); each tensor's report says
+    whether it was merged ("lora")."""
     if wtype not in (Q4_0, Q4_1):
         hint = " (q4_2 / q4_3 / mostly-q4_1-some-f16 are not supported)" if wtype in (4, 5, 6) else ""
         raise QuantizeError(f"invalid quantization type {wtype}{hint}: use 2 (q4_0) or 3 (q4_1)")
@@ -646,6 +762,8 @@ def quantize_model(in_path: str, out_path: str, wtype: int, fl: FlCuda | None = 
         if outtype is not None or vocab_dir is not None:
             raise QuantizeError(f"{in_path} is a model file: --outtype and --vocab-dir apply only to checkpoints")
         model = read_model(in_path)
+    adapter = read_lora(lora, model) if lora is not None else None
+    deltas = {d.base: d for d in adapter.deltas} if adapter else {}
     fl = fl or FlCuda()
     quantize_file = fl.fn("fl_dev_quantize_q4_file")
     bb = BLOCK_BYTES[wtype]
@@ -653,17 +771,25 @@ def quantize_model(in_path: str, out_path: str, wtype: int, fl: FlCuda | None = 
     staged = {t.name: int(np.prod(t.ne, dtype=np.int64)) * ELEM_BYTES[_src_type(t)] for t in mats}
     max_in = max(staged.values(), default=0)
     max_out = max((t.ne[0] // QK * t.ne[1] * bb for t in mats), default=0)
+    # the merged delta of a tensor ([M][K], f32 or f16) and, for an uncached adapter, its loraA and loraB back to back
+    by_name = {t.name: t for t in mats}
+    max_delta = max((int(np.prod(by_name[b].ne, dtype=np.int64)) * ELEM_BYTES[d.type] for b, d in deltas.items()), default=0)
+    max_ab = max((d.a.nbytes + d.b.nbytes for d in deltas.values() if d.a is not None), default=0)
+    quantize_lora = fl.fn("fl_dev_quantize_q4_file_lora") if deltas else None
 
     # a column-split shard, or a Hugging Face q / k matrix, lands in dev_cols first; then pitched device copies put it
     # into its column range of dev_in, or its rows into the converter's order
     max_cols = max((t.shards[0].nbytes for t in mats if t.split == SPLIT_COLUMNS or t.permute_heads), default=0)
 
     srcs = [np.memmap(p, dtype=np.uint8, mode="r") for p in model.paths]
+    lora_src = np.memmap(adapter.path, dtype=np.uint8, mode="r") if deltas else None
     dev_in = fl.alloc(max(max_in, 16))
     dev_cols = fl.alloc(max_cols) if max_cols else None
     dev_out = fl.alloc(max(max_out, 16))
     dev_hist = fl.alloc(16 * 8)
-    chunk = min(CHUNK_BYTES, max(max_in, 16))
+    dev_delta = fl.alloc(max_delta) if max_delta else None
+    dev_ab = fl.alloc(max_ab) if max_ab else None
+    chunk = min(CHUNK_BYTES, max(max_in, max_delta, max_ab, 16))
     stage = [_pinned(fl, chunk) for _ in range(2)]
     outbuf = _pinned(fl, max(max_out, 16))
     hist_host = _pinned(fl, 16 * 8)
@@ -676,7 +802,7 @@ def quantize_model(in_path: str, out_path: str, wtype: int, fl: FlCuda | None = 
 
     def record(i, t, new_type, size_new, hist):
         report["tensors"].append({"name": t.name, "ne": t.ne, "type": TYPE_NAMES[t.type], "new_type": TYPE_NAMES[new_type],
-                                  "size_org": t.nbytes, "size_new": size_new, "hist": hist})
+                                  "size_org": t.nbytes, "size_new": size_new, "hist": hist, "lora": t.name in deltas})
         report["total_size_org"] += t.nbytes
         report["total_size_new"] += size_new
         if verbose:
@@ -687,8 +813,25 @@ def quantize_model(in_path: str, out_path: str, wtype: int, fl: FlCuda | None = 
             else:
                 n_el = t.ne[0] * t.ne[1]
                 print(line + f"size = {t.nbytes / 1024 / 1024:8.2f} MB -> {size_new / 1024 / 1024:8.2f} MB | hist: "
-                      + " ".join(f"{h / n_el:5.3f}" for h in hist), flush=True)
+                      + " ".join(f"{h / n_el:5.3f}" for h in hist) + (" | + lora" if t.name in deltas else ""), flush=True)
 
+    def upload(src, offset: int, nbytes: int, dst: int) -> None:
+        """Copy src[offset:offset + nbytes] to device address dst through the two pinned chunks."""
+        nonlocal n_chunks
+        for off in range(0, nbytes, chunk):
+            n = min(chunk, nbytes - off)
+            s = n_chunks % 2
+            if stage_busy[s]:
+                fl.check(fl.lib.fl_event_sync(ev_stage[s]))      # the chunk staged there before is on the device
+            stage[s][1][:n] = src[offset + off:offset + off + n]
+            fl.check(fl.lib.fl_h2d(dst + off, stage[s][0], n))
+            fl.check(fl.lib.fl_event_record(ev_stage[s]))
+            stage_busy[s] = True
+            n_chunks += 1
+
+    if verbose and adapter:
+        print(f"lora: {adapter.path}: {'cached' if adapter.cached else 'uncached'}, r = {adapter.r}, alpha = {adapter.alpha}, "
+              f"{len(deltas)} tensors", flush=True)
     try:
         with open(out_path, "wb") as out:
             out.write(struct.pack("<II", GGJT_MAGIC, 1))
@@ -735,17 +878,7 @@ def quantize_model(in_path: str, out_path: str, wtype: int, fl: FlCuda | None = 
                 shards = t.shards[:1] if t.split == SPLIT_NONE else t.shards
                 for j, sh in enumerate(shards):
                     dst = dev_cols if t.split == SPLIT_COLUMNS or t.permute_heads else dev_in + j * sh.nbytes
-                    src = srcs[sh.part]
-                    for off in range(0, sh.nbytes, chunk):
-                        n = min(chunk, sh.nbytes - off)
-                        s = n_chunks % 2
-                        if stage_busy[s]:
-                            fl.check(fl.lib.fl_event_sync(ev_stage[s]))      # the chunk staged there before is on the device
-                        stage[s][1][:n] = src[sh.offset + off:sh.offset + off + n]
-                        fl.check(fl.lib.fl_h2d(dst + off, stage[s][0], n))
-                        fl.check(fl.lib.fl_event_record(ev_stage[s]))
-                        stage_busy[s] = True
-                        n_chunks += 1
+                    upload(srcs[sh.part], sh.offset, sh.nbytes, dst)
                     if t.split == SPLIT_COLUMNS:
                         w = sh.nbytes // t.ne[1]
                         fl.check(fl.lib.fl_d2d_2d(dev_in + j * w, w * len(shards), dev_cols, w, w, t.ne[1]))
@@ -757,14 +890,27 @@ def quantize_model(in_path: str, out_path: str, wtype: int, fl: FlCuda | None = 
                         for p in range(2):
                             fl.check(fl.lib.fl_d2d_2d(dev_in + (h * hd + p) * rb, 2 * rb, dev_cols + (h * hd + p * hd // 2) * rb,
                                                       rb, rb, hd // 2))
+                k, nrows = t.ne
+                d = deltas.get(t.name)
+                if d is not None and d.lora is not None:
+                    upload(lora_src, d.lora.offset, d.lora.nbytes, dev_delta)
+                elif d is not None:
+                    # B·A as the reference's ggml_mul_mat(loraA, loraB) computes it (ggml_vec_dot_f32 order): out[m][k] =
+                    # dot(loraA row k, loraB row m) over the rank, the [M][K] layout of the weight
+                    upload(lora_src, d.a.offset, d.a.nbytes, dev_ab)
+                    upload(lora_src, d.b.offset, d.b.nbytes, dev_ab + d.a.nbytes)
+                    fl.check(fl.lib.fl_dev_mul_mat_f32_ref(dev_ab, d.rank, k, dev_ab + d.a.nbytes, d.rank, nrows, d.rank,
+                                                           dev_delta, k))
                 # the previous quantised tensor goes to the file while this one's copies run
                 flush_pending()
-                k, nrows = t.ne
                 nbytes = k // QK * nrows * bb
-                # src 2: an f32 checkpoint's values as the converter's f16 file holds them
-                src = 2 if (_src_type(t), t.type) == (F32, F16) else _src_type(t)
                 fl.check(fl.lib.fl_dev_memset(dev_hist, 0, 16 * 8))
-                fl.check(quantize_file(wtype, src, dev_in, dev_out, k, nrows, dev_hist))
+                if d is None:
+                    # src 2: an f32 checkpoint's values as the converter's f16 file holds them
+                    src = 2 if (_src_type(t), t.type) == (F32, F16) else _src_type(t)
+                    fl.check(quantize_file(wtype, src, dev_in, dev_out, k, nrows, dev_hist))
+                else:
+                    fl.check(quantize_lora(wtype, _merge_src(t), dev_in, d.type, dev_delta, dev_out, k, nrows, dev_hist))
                 fl.check(fl.lib.fl_d2h(outbuf[0], dev_out, nbytes))
                 fl.check(fl.lib.fl_d2h(hist_host[0], dev_hist, 16 * 8))
                 fl.check(fl.lib.fl_event_record(ev_out))
@@ -776,10 +922,10 @@ def quantize_model(in_path: str, out_path: str, wtype: int, fl: FlCuda | None = 
             fl.lib.fl_event_destroy(e)
         for p, _ in stage + [outbuf, hist_host]:
             fl.lib.fl_host_free_pinned(p)
-        for d in (dev_in, dev_cols, dev_out, dev_hist):
+        for d in (dev_in, dev_cols, dev_out, dev_hist, dev_delta, dev_ab):
             if d is not None:
                 fl.free(d)
-        del srcs
+        del srcs, lora_src
     if verbose:
         tot = sum(report["hist"]) or 1
         print(f"model size  = {report['total_size_org'] / 1024 / 1024:8.2f} MB")
@@ -788,12 +934,15 @@ def quantize_model(in_path: str, out_path: str, wtype: int, fl: FlCuda | None = 
     return report
 
 
-USAGE = """usage: python -m fastllama_b200.quantize IN OUT TYPE [--outtype f16|f32] [--vocab-dir DIR]
+USAGE = """usage: python -m fastllama_b200.quantize IN OUT TYPE [--outtype f16|f32] [--vocab-dir DIR] [--lora ADAPTER]
   TYPE = 2 - q4_0, 3 - q4_1
   IN: an f16 / f32 model file (a model in parts: part 0; the others are read from IN.1, IN.2, ...), or a
       PyTorch / safetensors checkpoint (a directory, or its first file), quantised as the f16 (--outtype f16, the
       default) or f32 file the reference's scripts/convert.py writes from it; tokenizer.model is read from
-      --vocab-dir, else from beside the checkpoint, else from its parent directory"""
+      --vocab-dir, else from beside the checkpoint, else from its parent directory
+  --lora ADAPTER: a LoRA adapter as the reference's scripts/convert-lora-to-ggml.py writes it (cached f32, uncached
+      f32 or cached f16), merged into the f16 / f32 weights before they are quantised: OUT is the reference tool's
+      file for the model after the reference's attach_lora, and needs no adapter at load"""
 
 
 def main(argv=None) -> int:
@@ -802,7 +951,7 @@ def main(argv=None) -> int:
     while argv:
         a = argv.pop(0)
         key, eq, val = a.partition("=")
-        if key in ("--outtype", "--vocab-dir"):
+        if key in ("--outtype", "--vocab-dir", "--lora"):
             if not eq:
                 if not argv:
                     print(USAGE, file=sys.stderr)

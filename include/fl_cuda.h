@@ -119,6 +119,14 @@ int fl_dev_quantize_q4(int type, const float *x, void *y, int k, int nrows);
  * ggml_quantize_chunk reports.  Asynchronous on the library stream, like every fl_dev_* call. */
 int fl_dev_quantize_q4_file(int type, int src_type, const void *x_dev, void *y_dev, int k, int nrows,
                             unsigned long long *hist_dev);
+/* fl_dev_quantize_q4_file with a LoRA delta merged into each element before the q4 rounding, as the reference's
+ * attach_lora merges an adapter into an unquantised model (ggml_add_inplace, lib/ggml.c:6259-6412).  delta_dev holds
+ * nrows rows of k elements in x's layout: delta_type 0 = f32, 1 = f16, or -1 with delta_dev NULL for no delta (then
+ * this is fl_dev_quantize_q4_file, bit for bit).  The merge rule is the file's: src_type 0 (f32 file) and 3 (f16 data
+ * of an f32 file, as an f16 checkpoint converted to f32) add in fp32, w + d; src_type 1 (f16 file) and 2 (f32 rounded
+ * to f16) round the fp32 sum to f16, fp16_rn(w + fp32(d)).  An f16 delta with src_type 0 or 3 is an error. */
+int fl_dev_quantize_q4_file_lora(int type, int src_type, const void *x_dev, int delta_type, const void *delta_dev, void *y_dev, int k,
+                                 int nrows, unsigned long long *hist_dev);
 
 /* ---- attach_lora / detach_lora on the device (reference lib/llama.cpp:697-944; SURVEY.md section 8 row f4) ----
  * fl_dev_quantize_q4_simd: device-resident fl_quantize_rows_q4_simd.
